@@ -720,6 +720,11 @@ class Emitter:
         else:
             ranges = [(0, len(self.layout), 0)]
             out.append(" ".join(f"o_[{j}] = 0u;" for j in range(W)))
+        changed = set()         # packed words this site may write (the others are the parent's)
+        for first, cnt, bitpos in ranges:
+            width = sum(self.layout[s][1] for s in range(first, first + cnt))
+            if width:
+                changed.update(range(bitpos >> 5, (bitpos + width - 1) // 32 + 1))
         for first, cnt, bitpos in ranges:
             for s in range(first, first + cnt):
                 off, width, bias = self.layout[s]
@@ -740,7 +745,13 @@ class Emitter:
                 st += " }"
                 out.append(st)
                 bitpos += width
-        out.append(f"TLAG_SL_EMITW({aid}, o_); }}")
+        # A successor equal to its parent (an action that is enabled but changes nothing) is counted and dropped: the
+        # parent is a stored state, so the seen-set probe would only find it there.  The test reads registers only.
+        diff = " | ".join(f"(o_[{j}] ^ in_[{j}])" for j in sorted(changed if dirty > 0 else range(W)))
+        if diff:
+            out.append(f"if (TLAG_SL_SKIPSELF && ({diff}) == 0u) TLAG_SL_GEN(); else TLAG_SL_EMITW({aid}, o_); }}")
+        else:
+            out.append(f"if (TLAG_SL_SKIPSELF) TLAG_SL_GEN(); else TLAG_SL_EMITW({aid}, o_); }}")
         return "\n    ".join(out)
 
     def unpack_code(self, live_in=None):
@@ -834,6 +845,8 @@ class Emitter:
             f"#define TLAG_NATIVE_CPOOL_FNV 0x{self._cpool_fnv():016x}ULL  /* ... over the constant pool (folded into the code) */",
             f"#define TLAG_SL_W {self.W}", f"#define TLAG_SL_USZ {self.usz}", f"#define TLAG_SL_FRAME {self.frame}",
             f"#define TLAG_SL_SCALAR {1 if self.scalar else 0}",
+            "#ifndef TLAG_SL_SKIPSELF        /* scalar form: drop successors equal to their parent (CUDA: a run-time switch) */",
+            "#define TLAG_SL_SKIPSELF 1", "#endif",
             f"#define TLAG_SL_NINV {n_inv_prog}", f"#define TLAG_SL_NNEXT {len(nsegs)}",
             "#define TLAG_SL_INV_LIST(X) " + " ".join(f"X({j})" for j in range(n_inv_prog)),
             "#define TLAG_SL_NEXT_LIST(X) " + " ".join(f"X({j})" for j in range(len(nsegs))),

@@ -41,6 +41,7 @@ struct DevParams {
   int owner_words;                  // trailing packed words the ownership hash covers (tlag_owner_k; 2 = clustering key)
   uint32_t* send; unsigned long long region_cap; int n_ranks; int rank;
   unsigned long long* sent_cache; unsigned long long sent_mask;   // direct-mapped filter of fingerprints already routed
+  int skip_self;                    // sliced build: a successor equal to its parent is counted, never fingerprinted or probed
 };
 
 // ---- peer-memory exchange (tlag_engine.cu: k_push / k_insert_inbox) ----
@@ -111,6 +112,8 @@ __device__ __forceinline__ void report_min(unsigned long long* slot, unsigned lo
 // A translation unit that holds slices defines TLAG_SLICED_DEFS (the generated header with the model's constants) before
 // including this file, then the slice functions, then TLAG_SL_KERNEL_INV(j) / TLAG_SL_KERNEL_NEXT(j) for its slices.
 #ifdef TLAG_SLICED_DEFS
+// the scalar form's emit sites test this before they hand a successor equal to its parent to TLAG_SL_EMITW
+#define TLAG_SL_SKIPSELF (cx->p->skip_self)
 #include TLAG_SLICED_DEFS
 struct tlag_sl_cx {
   const DevParams* p;

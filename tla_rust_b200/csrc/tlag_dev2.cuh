@@ -79,6 +79,8 @@ static __device__ __noinline__ void sl_emit_frame(tlag_sl_cx* cx, const int32_t*
     report_min(&p.ctr->viol_trap, (cx->idx << 20) | (2ULL << 16) | (unsigned)((ov - 1) & 0xFFFF));
     return;
   }
+  // (no self-loop test here: comparing every word with the parent's row in memory cost raft 1 % of its wave time and
+  // saved SSI none; the scalar form tests its registers, compile/sliced.py: emit_stmt)
   sl_emit_words(cx, aid, succ);
 }
 

@@ -1042,6 +1042,13 @@ extern "C" int tlag_create(const tlag_model* m, tlag_engine** out) {
   e->p.states = e->d_states; e->p.parent = e->d_parent; e->p.meta = e->d_meta; e->p.cap_states = cap;
   e->p.ctr = e->d_ctr; e->p.flags = m->flags; e->p.n_inv = (int)m->n_invariants;
   e->p.n_ranks = 1; e->p.rank = 0; e->p.owner_words = 2;
+  // Sliced build: a successor whose packed words equal its parent's is counted (generated, has-a-successor) and dropped
+  // before the fingerprint and the seen-set probe, which would always find the parent there.  Paxos' enabled-but-
+  // unchanging actions make 65 % of its successors self-loops.  TLAG_SL_SKIPSELF=0 probes them like any other successor.
+  {
+    const char* s_ = getenv("TLAG_SL_SKIPSELF");
+    e->p.skip_self = (s_ && *s_) ? (atoi(s_) != 0) : 1;
+  }
   unsigned log2 = m->table_slots_log2 ? m->table_slots_log2 : 22;
   int r = alloc_table(e, log2);
   if (r) return r;
