@@ -42,6 +42,7 @@ struct DevParams {
   uint32_t* send; unsigned long long region_cap; int n_ranks; int rank;
   unsigned long long* sent_cache; unsigned long long sent_mask;   // direct-mapped filter of fingerprints already routed
   int skip_self;                    // sliced build: a successor equal to its parent is counted, never fingerprinted or probed
+  int stage;                        // sliced build, scalar form: cap on the per-warp staging slots used (0: none, all direct)
 };
 
 // ---- peer-memory exchange (tlag_engine.cu: k_push / k_insert_inbox) ----
@@ -107,8 +108,8 @@ __device__ __forceinline__ void report_min(unsigned long long* slot, unsigned lo
 // k_sl_next_<j> one disjunct of Next, each over the whole frontier, one thread per state.  All warps of a launch run
 // the same few KB of straight-line code (the whole-program compiled form of round 1 lost to the interpreter on
 // instruction-cache misses: 354 KB of code, every warp somewhere else); divergence inside a slice is the hardware's
-// (compiler-placed reconvergence) instead of a min-pc election per block; a successor is packed, fingerprinted and
-// inserted where it is produced, with opportunistic warp aggregation of the tail-counter atomics.
+// (compiler-placed reconvergence) instead of a min-pc election per block; a successor is packed where it is produced,
+// then staged for a probe by the whole warp (scalar form) or fingerprinted and inserted there (array form).
 // A translation unit that holds slices defines TLAG_SLICED_DEFS (the generated header with the model's constants) before
 // including this file, then the slice functions, then TLAG_SL_KERNEL_INV(j) / TLAG_SL_KERNEL_NEXT(j) for its slices.
 #ifdef TLAG_SLICED_DEFS
@@ -122,6 +123,9 @@ struct tlag_sl_cx {
   unsigned long long gen;
   unsigned nsucc;
   int phase;                        // 0 = invariant slice, 1 = slice of Next
+#if TLAG_SL_SCALAR                  // (only the scalar form stages: the array form's kernels are left as they were)
+  unsigned stage_cap;               // staging slots this launch may use per warp (0: every successor goes direct)
+#endif
 };
 
 #ifndef TLAG_SL_BLOCK
@@ -134,7 +138,51 @@ struct tlag_sl_cx {
 static __device__ __noinline__ void sl_emit_words(tlag_sl_cx* cx, int aid, const uint32_t* o);
 static __device__ __noinline__ void sl_emit_frame(tlag_sl_cx* cx, const int32_t* f, int aid, int dirty);
 #define TLAG_SL_EMIT(aid, dirty) sl_emit_frame(cx, f, (aid), (dirty))
+
+// Per-warp staging (scalar form, Next kernels, not in route mode).  An emit site puts its successor into a slot of its
+// warp's buffer; the whole warp later fingerprints and probes the staged successors together (sl_flush, tlag_dev2.cuh),
+// instead of every group of lanes that reaches a site waiting on its own seen-set round trip inside divergent code.
+// Budget: 3.5 KB a warp, 28 KB a 256-thread CTA, so that 4 CTAs per SM take 112 KB of the 228 KB of shared memory.
+// A slot holds the W packed words, the parent index and the meta word; at fewer than 32 slots (W > 25) nothing is staged.
+#define TLAG_SL_STAGE_BYTES 3584
+#define TLAG_SL_STAGE_SLOTS ((TLAG_SL_STAGE_BYTES / (4 * (TLAG_SL_W + 2)) / 32) * 32)
+#if TLAG_SL_SCALAR && TLAG_SL_STAGE_SLOTS >= 32
+#define TLAG_SL_STAGED 1
+// word-major: word k of slot s of warp v at [v][k][s], so that the lanes of an emit site (consecutive slots) and of a
+// flush (slots lane, lane + 32, ...) hit distinct banks; the row is one word longer than the slots so that the flush's
+// copy into the store (consecutive words of one slot on consecutive lanes) does too.  Words W, W + 1: parent, meta.
+static __shared__ uint32_t tlag_sl_stage[TLAG_SL_BLOCK / 32][TLAG_SL_W + 2][TLAG_SL_STAGE_SLOTS + 1];
+static __shared__ unsigned tlag_sl_fill[TLAG_SL_BLOCK / 32];     // slots taken; may run past the cap (those went direct)
+static __shared__ unsigned short tlag_sl_row[TLAG_SL_BLOCK / 32][TLAG_SL_STAGE_SLOTS];   // flush: new row -> slot
+
+static __device__ __forceinline__ void sl_stage_words(tlag_sl_cx* cx, int aid, const uint32_t* o) {
+  constexpr int W = TLAG_SL_W;
+  const unsigned lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  // divergent groups of one warp can interleave here: slots are taken with one shared atomic per arriving group
+  const unsigned am = __activemask();
+  const int leader = __ffs((int)am) - 1;
+  unsigned base = 0;
+  if ((int)lane == leader) base = atomicAdd(&tlag_sl_fill[warp], (unsigned)__popc(am));
+  base = __shfl_sync(am, base, leader);
+  const unsigned s = base + (unsigned)__popc(am & lanemask_lt());
+  if (s < cx->stage_cap) {
+    cx->nsucc++; cx->gen++;
+#pragma unroll
+    for (int k = 0; k < W; ++k) tlag_sl_stage[warp][k][s] = o[k];
+    tlag_sl_stage[warp][W][s] = (uint32_t)cx->idx;
+    tlag_sl_stage[warp][W + 1][s] = ((uint32_t)aid << 8) | (uint32_t)(cx->p->rank & 0xFF);
+  } else {
+    // buffer full: probe here, as without staging (a copy, so that the site's words can stay in registers)
+    uint32_t w[W];
+#pragma unroll
+    for (int k = 0; k < W; ++k) w[k] = o[k];
+    sl_emit_words(cx, aid, w);
+  }
+}
+#define TLAG_SL_EMITW(aid, o) sl_stage_words(cx, (aid), (o))
+#else
 #define TLAG_SL_EMITW(aid, o) sl_emit_words(cx, (aid), (o))
+#endif
 #define TLAG_SL_GEN() do { cx->nsucc++; cx->gen++; } while (0)
 #define TLAG_SL_ASSERT(id) report_min(&cx->p->ctr->viol_assert, (cx->idx << 20) | (unsigned)((id) & 0xFFFFF))
 #define TLAG_SL_INVF(i) do { if (cx->phase == 0) report_min(&cx->p->ctr->viol_inv, (cx->idx << 20) | (unsigned)((i) & 0xFFFFF)); } while (0)

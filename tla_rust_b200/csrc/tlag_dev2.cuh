@@ -85,25 +85,120 @@ static __device__ __noinline__ void sl_emit_frame(tlag_sl_cx* cx, const int32_t*
 }
 
 
-// One thread per frontier state (grid-stride).  FN: the slice function of this kernel.
+#ifdef TLAG_SL_STAGED
+// The whole warp: fingerprint the staged successors and probe the seen-set for them, then append the new ones to the
+// store as one contiguous run (one tail atomic, coalesced stores).  Semantics as sl_emit_words: a row past the store's
+// capacity is counted in n_states and reported as an overflow, a full table as table_full.
+static __device__ __forceinline__ void sl_flush(const DevParams& p, unsigned cap) {
+  constexpr int W = TLAG_SL_W, R = TLAG_SL_STAGE_SLOTS / 32;
+  const unsigned lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  __syncwarp();
+  const unsigned n = min(tlag_sl_fill[warp], cap);
+  unsigned long long fp[R], cur[R];
+  // every table load of this lane is issued before any is examined: R probes in flight per lane
+#pragma unroll
+  for (int r = 0; r < R; ++r) {
+    const unsigned s = r * 32 + lane;
+    fp[r] = 0; cur[r] = 0;
+    if (s < n) {
+      uint32_t w[W];
+#pragma unroll
+      for (int k = 0; k < W; ++k) w[k] = tlag_sl_stage[warp][k][s];
+      fp[r] = tlag_fingerprint(w, W);
+      cur[r] = __ldcv(&p.table[fp[r] & p.mask]);
+    }
+  }
+  unsigned total = 0;
+#pragma unroll
+  for (int r = 0; r < R; ++r) {
+    int ins = 0;
+    if (r * 32 + lane < n && cur[r] != fp[r]) {
+      // first slot empty: claim it; taken by another state: the whole probe (seen_insert) from the start
+      const unsigned long long old = cur[r] ? cur[r] : atomicCAS(&p.table[fp[r] & p.mask], 0ULL, fp[r]);
+      ins = old == 0ULL ? 1 : (old == fp[r] ? 0 : seen_insert(p.table, p.mask, fp[r]));
+      if (ins < 0) { atomicExch(&p.ctr->table_full, 1ULL); ins = 0; }
+    }
+    const unsigned m = __ballot_sync(0xffffffffu, ins > 0);
+    if (ins > 0) tlag_sl_row[warp][total + __popc(m & lanemask_lt())] = (unsigned short)(r * 32 + lane);
+    total += __popc(m);
+  }
+  if (total) {
+    unsigned long long base = 0;
+    if (lane == 0) base = atomicAdd(&p.ctr->n_states, (unsigned long long)total);
+    base = __shfl_sync(0xffffffffu, base, 0);
+    __syncwarp();
+    for (unsigned t = lane; t < total * W; t += 32) {
+      const unsigned row = t / W, k = t - row * W;
+      const unsigned long long pos = base + row;
+      if (pos < p.cap_states) p.states[pos * W + k] = tlag_sl_stage[warp][k][tlag_sl_row[warp][row]];
+    }
+    for (unsigned row = lane; row < total; row += 32) {
+      const unsigned long long pos = base + row;
+      const unsigned s = tlag_sl_row[warp][row];
+      if (pos < p.cap_states) {
+        p.parent[pos] = tlag_sl_stage[warp][W][s];
+        p.meta[pos] = tlag_sl_stage[warp][W + 1][s];
+      } else {
+        atomicExch(&p.ctr->store_overflow, 1ULL);
+      }
+    }
+  }
+  __syncwarp();
+  if (lane == 0) tlag_sl_fill[warp] = 0;
+  __syncwarp();
+}
+#endif
+
+// One thread per frontier state (grid-stride).  A staged Next kernel strides over whole warps, so that a warp is
+// converged at the bottom of every iteration and can flush its staged successors together; the other kernels keep one
+// lane per state.  FN: the slice function of this kernel.
 template <int PHASE, typename FN>
 __device__ __forceinline__ void sl_run(const DevParams& p, unsigned long long lo, unsigned long long hi, FN fn) {
   constexpr int W = TLAG_SL_W;
+#ifdef TLAG_SL_STAGED
+  constexpr bool staged = PHASE == 1;
+#else
+  constexpr bool staged = false;
+#endif
   tlag_sl_cx cxs;
   tlag_sl_cx* cx = &cxs;
   cx->p = &p; cx->gen = 0; cx->phase = PHASE;
-  const unsigned long long stride = (unsigned long long)gridDim.x * blockDim.x;
-  for (unsigned long long idx = lo + (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; idx < hi; idx += stride) {
-    const uint32_t* src = p.states + idx * (unsigned long long)W;
-    cx->idx = idx; cx->nsucc = 0;
-    // the slice unpacks the slots it reads (liveness, compile/sliced.py) straight out of these registers
-    uint32_t in_[W];
-#pragma unroll
-    for (int i = 0; i < W; ++i) in_[i] = src[i];
-    cx->src = src;                 // (the global row: taking the address of in_ would force it out of registers)
-    fn(p.cpool, in_, cx);
-    if (PHASE == 1 && cx->nsucc && p.succ_flag) p.succ_flag[idx - lo] = 1;
+  const unsigned lane = threadIdx.x & 31;
+#ifdef TLAG_SL_STAGED
+  cx->stage_cap = 0;
+  if (staged) {
+    // route mode keeps the direct path: its send regions and sent-cache have their own ordering
+    cx->stage_cap = p.route ? 0u : min((unsigned)p.stage, (unsigned)TLAG_SL_STAGE_SLOTS);
+    if (lane == 0) tlag_sl_fill[threadIdx.x >> 5] = 0;
+    __syncwarp();
   }
+#endif
+  const unsigned long long stride = (unsigned long long)gridDim.x * blockDim.x;
+  for (unsigned long long i0 = lo + (unsigned long long)blockIdx.x * blockDim.x + (staged ? threadIdx.x & ~31u : threadIdx.x);
+       i0 < hi; i0 += stride) {
+    const unsigned long long idx = staged ? i0 + lane : i0;
+    if (!staged || idx < hi) {
+      const uint32_t* src = p.states + idx * (unsigned long long)W;
+      cx->idx = idx; cx->nsucc = 0;
+      // the slice unpacks the slots it reads (liveness, compile/sliced.py) straight out of these registers
+      uint32_t in_[W];
+#pragma unroll
+      for (int i = 0; i < W; ++i) in_[i] = src[i];
+      cx->src = src;                 // (the global row: taking the address of in_ would force it out of registers)
+      fn(p.cpool, in_, cx);
+      if (PHASE == 1 && cx->nsucc && p.succ_flag) p.succ_flag[idx - lo] = 1;
+    }
+#ifdef TLAG_SL_STAGED
+    // flush at half full: the next iteration's successors then usually fit
+    if (staged) {
+      __syncwarp();
+      if (tlag_sl_fill[threadIdx.x >> 5] >= cx->stage_cap / 2) sl_flush(p, cx->stage_cap);
+    }
+#endif
+  }
+#ifdef TLAG_SL_STAGED
+  if (staged) sl_flush(p, cx->stage_cap);
+#endif
   // generated counter: warp reduce, one atomic per warp
   unsigned long long g = cx->gen;
   if (PHASE == 1) {

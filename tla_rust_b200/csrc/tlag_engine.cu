@@ -13,6 +13,7 @@
 // (SURVEY.md §2b; all external to /root/reference, which only fixes the CLI contract
 // Makefile:6-7 and the output format README.md:267-321).
 #include <cuda_runtime.h>
+#include <limits.h>
 #include <stdint.h>
 #include <stdio.h>
 #include <string.h>
@@ -1048,6 +1049,13 @@ extern "C" int tlag_create(const tlag_model* m, tlag_engine** out) {
   {
     const char* s_ = getenv("TLAG_SL_SKIPSELF");
     e->p.skip_self = (s_ && *s_) ? (atoi(s_) != 0) : 1;
+  }
+  // Sliced build, scalar form: successors are staged per warp and probed by the whole warp together (tlag_dev.cuh,
+  // TLAG_SL_STAGED).  TLAG_SL_STAGE=n caps the slots a warp uses below the compiled number, so that a test can make the
+  // buffer fill up and the direct path run (0: every successor is probed where it is produced).  Not a tuning knob.
+  {
+    const char* s_ = getenv("TLAG_SL_STAGE");
+    e->p.stage = (s_ && *s_) ? (atoi(s_) > 0 ? atoi(s_) : 0) : INT_MAX;
   }
   unsigned log2 = m->table_slots_log2 ? m->table_slots_log2 : 22;
   int r = alloc_table(e, log2);

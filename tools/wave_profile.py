@@ -38,6 +38,9 @@ def switches():
     v = os.environ.get("TLAG_SL_SKIPSELF", "")
     lead = re.match(r"\s*[+-]?\d+", v)            # as tlag_create reads it: unset or empty = on, else atoi() != 0
     out["TLAG_SL_SKIPSELF"] = "1" if not v or (lead and int(lead.group()) != 0) else "0"
+    v = os.environ.get("TLAG_SL_STAGE", "")        # unset or empty = every compiled staging slot, else max(0, atoi())
+    lead = re.match(r"\s*[+-]?\d+", v)
+    out["TLAG_SL_STAGE"] = "all" if not v else str(max(0, int(lead.group())) if lead else 0)
     return out
 
 
