@@ -1,6 +1,7 @@
 // tlag_dev.cuh -- device-side definitions shared by the engine (tlag_engine.cu) and by the translation units of a
 // sliced native build (tla_rust_b200/compile/sliced.py writes one .cu per group of slices; they are compiled in
-// parallel and linked into one library): counters, kernel parameters, the seen-set probe, and the slice runtime.
+// parallel and linked into one library): counters, kernel parameters, the seen-set probe, the appends to the store and
+// to the send regions, and the slice runtime.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -93,10 +94,79 @@ __device__ __forceinline__ int seen_insert(unsigned long long* table, unsigned l
   return -1;
 }
 
+// seen_insert for a caller that has already loaded the home slot (table[fp & mask]) as cur, so that it can keep several
+// such loads in flight: an empty slot is claimed with a CAS, one that holds another state runs the whole probe
+__device__ __forceinline__ int seen_insert_at(unsigned long long* table, unsigned long long mask, unsigned long long fp,
+                                              unsigned long long cur) {
+  if (cur == fp) return 0;
+  if (cur == 0ULL) {
+    const unsigned long long old = atomicCAS(&table[fp & mask], 0ULL, fp);
+    if (old == 0ULL) return 1;
+    if (old == fp) return 0;
+  }
+  return seen_insert(table, mask, fp);
+}
+
+// the result of a probe, with a full table (-1) reported in table_full: 1 if the state is new, else 0
+__device__ __forceinline__ int seen_report(Counters* ctr, int ins) {
+  if (ins < 0) { atomicExch(&ctr->table_full, 1ULL); return 0; }
+  return ins;
+}
+
 __device__ __forceinline__ unsigned lanemask_lt() {
   unsigned m;
   asm("mov.u32 %0, %%lanemask_lt;" : "=r"(m));
   return m;
+}
+
+// meta word of a stored state: the action that produced it, and the rank that expanded its parent (whose store the
+// parent index points into)
+__device__ __forceinline__ uint32_t tlag_meta(int aid, int rank) { return ((uint32_t)aid << 8) | (uint32_t)(rank & 0xFF); }
+
+// Appends a new state to the tail of the store.  Only the lanes of `group` call it, each with a new state: one tail
+// atomic for the group, rows in lane order.  A row past cap_states is still counted in n_states (the host sizes the
+// rerun of the level from it) and is reported in store_overflow.
+__device__ __forceinline__ void store_append(const DevParams& p, unsigned group, const uint32_t* w, int W, uint32_t parent,
+                                             uint32_t meta) {
+  const int leader = __ffs((int)group) - 1;
+  unsigned long long base = 0;
+  if ((int)(threadIdx.x & 31) == leader) base = atomicAdd(&p.ctr->n_states, (unsigned long long)__popc(group));
+  base = __shfl_sync(group, base, leader);
+  const unsigned long long pos = base + (unsigned long long)__popc(group & lanemask_lt());
+  if (pos < p.cap_states) {
+    uint32_t* dst = p.states + pos * (unsigned long long)W;
+    for (int i = 0; i < W; ++i) dst[i] = w[i];
+    p.parent[pos] = parent;
+    p.meta[pos] = meta;
+  } else {
+    atomicExch(&p.ctr->store_overflow, 1ULL);
+  }
+}
+
+// Route mode: appends a successor that `owner` holds to that rank's send region (W words, parent, meta), with one
+// atomic per group of lanes present that route to the same owner.  A successor whose fingerprint this rank has already
+// routed is known to its owner and is dropped (direct-mapped exact-compare cache: a miss only costs a redundant record).
+// The cache slot is written only once the record is in the send region, so a chunk that is re-run after a region
+// overflow finds none of its dropped records there.
+__device__ __forceinline__ void route_append(const DevParams& p, const uint32_t* w, int W, unsigned long long fp, int owner,
+                                             uint32_t parent, uint32_t meta) {
+  unsigned long long* cslot = p.sent_cache ? p.sent_cache + (fp & p.sent_mask) : nullptr;
+  if (cslot && __ldcv(cslot) == fp) return;
+  const unsigned peers = __match_any_sync(__activemask(), owner);
+  const int leader = __ffs((int)peers) - 1;
+  unsigned long long base = 0;
+  if ((int)(threadIdx.x & 31) == leader) base = atomicAdd(&p.ctr->send_count[owner], (unsigned long long)__popc(peers));
+  base = __shfl_sync(peers, base, leader);
+  const unsigned long long pos = base + (unsigned long long)__popc(peers & lanemask_lt());
+  if (pos < p.region_cap) {
+    uint32_t* dst = p.send + ((unsigned long long)owner * p.region_cap + pos) * (unsigned long long)(W + 2);
+    for (int i = 0; i < W; ++i) dst[i] = w[i];
+    dst[W] = parent;
+    dst[W + 1] = meta;
+    if (cslot) *cslot = fp;
+  } else {
+    atomicExch(&p.ctr->route_overflow, 1ULL);
+  }
 }
 
 __device__ __forceinline__ void report_min(unsigned long long* slot, unsigned long long key) {
@@ -170,7 +240,7 @@ static __device__ __forceinline__ void sl_stage_words(tlag_sl_cx* cx, int aid, c
 #pragma unroll
     for (int k = 0; k < W; ++k) tlag_sl_stage[warp][k][s] = o[k];
     tlag_sl_stage[warp][W][s] = (uint32_t)cx->idx;
-    tlag_sl_stage[warp][W + 1][s] = ((uint32_t)aid << 8) | (uint32_t)(cx->p->rank & 0xFF);
+    tlag_sl_stage[warp][W + 1][s] = tlag_meta(aid, cx->p->rank);
   } else {
     // buffer full: probe here, as without staging (a copy, so that the site's words can stay in registers)
     uint32_t w[W];

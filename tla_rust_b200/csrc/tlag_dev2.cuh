@@ -11,53 +11,14 @@ static __device__ __noinline__ void sl_emit_words(tlag_sl_cx* cx, int aid, const
 #pragma unroll
   for (int i = 0; i < W; ++i) w[i] = o[i];
   const unsigned long long fp = tlag_fingerprint(w, W);
-  const unsigned lane = threadIdx.x & 31;
   // route mode: a successor this rank owns itself never leaves the GPU (1/N of the records)
   const int owner = p.route ? (int)tlag_owner_k(w, W, (uint32_t)p.n_ranks, p.owner_words) : p.rank;
   if (!p.route || owner == p.rank) {
-    int ins = seen_insert(p.table, p.mask, fp);
-    if (ins < 0) { atomicExch(&p.ctr->table_full, 1ULL); ins = 0; }
-    if (ins > 0) {
-      // warp-aggregated tail allocation over whichever lanes arrived here together
-      const unsigned am = __activemask();
-      const int leader = __ffs((int)am) - 1;
-      unsigned long long base = 0;
-      if ((int)lane == leader) base = atomicAdd(&p.ctr->n_states, (unsigned long long)__popc(am));
-      base = __shfl_sync(am, base, leader);
-      const unsigned long long pos = base + (unsigned long long)__popc(am & lanemask_lt());
-      if (pos < p.cap_states) {
-        uint32_t* dst = p.states + pos * (unsigned long long)W;
-#pragma unroll
-        for (int i = 0; i < W; ++i) dst[i] = w[i];
-        p.parent[pos] = (uint32_t)cx->idx;
-        p.meta[pos] = ((uint32_t)aid << 8) | (uint32_t)(p.rank & 0xFF);
-      } else {
-        atomicExch(&p.ctr->store_overflow, 1ULL);
-      }
-    }
+    // the tail allocation is aggregated over whichever lanes arrived here together
+    if (seen_report(p.ctr, seen_insert(p.table, p.mask, fp)))
+      store_append(p, __activemask(), w, W, (uint32_t)cx->idx, tlag_meta(aid, p.rank));
   } else {
-    // A successor whose fingerprint this rank has already routed is known to its owner (direct-mapped exact-compare
-    // cache).  The slot is written only once the record is in the send region, so a chunk that is re-run after a
-    // region overflow loses nothing.
-    unsigned long long* cslot = p.sent_cache ? p.sent_cache + (fp & p.sent_mask) : nullptr;
-    if (cslot && __ldcv(cslot) == fp) return;
-    const unsigned am = __activemask();
-    const unsigned peers = __match_any_sync(am, owner);
-    const int leader = __ffs((int)peers) - 1;
-    unsigned long long base = 0;
-    if ((int)lane == leader) base = atomicAdd(&p.ctr->send_count[owner], (unsigned long long)__popc(peers));
-    base = __shfl_sync(peers, base, leader);
-    const unsigned long long pos = base + (unsigned long long)__popc(peers & lanemask_lt());
-    if (pos < p.region_cap) {
-      uint32_t* dst = p.send + ((unsigned long long)owner * p.region_cap + pos) * (unsigned long long)(W + 2);
-#pragma unroll
-      for (int i = 0; i < W; ++i) dst[i] = w[i];
-      dst[W] = (uint32_t)cx->idx;
-      dst[W + 1] = ((uint32_t)aid << 8) | (uint32_t)(p.rank & 0xFF);
-      if (cslot) *cslot = fp;
-    } else {
-      atomicExch(&p.ctr->route_overflow, 1ULL);
-    }
+    route_append(p, w, W, fp, owner, (uint32_t)cx->idx, tlag_meta(aid, p.rank));
   }
 }
 
@@ -111,13 +72,7 @@ static __device__ __forceinline__ void sl_flush(const DevParams& p, unsigned cap
   unsigned total = 0;
 #pragma unroll
   for (int r = 0; r < R; ++r) {
-    int ins = 0;
-    if (r * 32 + lane < n && cur[r] != fp[r]) {
-      // first slot empty: claim it; taken by another state: the whole probe (seen_insert) from the start
-      const unsigned long long old = cur[r] ? cur[r] : atomicCAS(&p.table[fp[r] & p.mask], 0ULL, fp[r]);
-      ins = old == 0ULL ? 1 : (old == fp[r] ? 0 : seen_insert(p.table, p.mask, fp[r]));
-      if (ins < 0) { atomicExch(&p.ctr->table_full, 1ULL); ins = 0; }
-    }
+    const int ins = r * 32 + lane < n ? seen_report(p.ctr, seen_insert_at(p.table, p.mask, fp[r], cur[r])) : 0;
     const unsigned m = __ballot_sync(0xffffffffu, ins > 0);
     if (ins > 0) tlag_sl_row[warp][total + __popc(m & lanemask_lt())] = (unsigned short)(r * 32 + lane);
     total += __popc(m);

@@ -241,53 +241,13 @@ k_wave(DevParams p, unsigned long long lo, unsigned long long hi) {
         }
       }
       if (MODE == 0) {
-        int ins = has ? seen_insert(p.table, p.mask, fp) : 0;
-        if (ins < 0) { atomicExch(&p.ctr->table_full, 1ULL); ins = 0; }
-        const bool isnew = ins > 0;
+        const bool isnew = has && seen_report(p.ctr, seen_insert(p.table, p.mask, fp));
         const unsigned m = __ballot_sync(0xffffffffu, isnew);
-        if (m) {
-          const int leader = __ffs((int)m) - 1;
-          unsigned long long base = 0;
-          if ((int)lane == leader) base = atomicAdd(&p.ctr->n_states, (unsigned long long)__popc(m));
-          base = __shfl_sync(0xffffffffu, base, leader);
-          if (isnew) {
-            const unsigned long long pos = base + (unsigned long long)__popc(m & lanemask_lt());
-            if (pos < p.cap_states) {
-              uint32_t* dst = p.states + pos * (unsigned long long)W;
-              for (int i = 0; i < W; ++i) dst[i] = succ[i];
-              p.parent[pos] = (uint32_t)idx;
-              p.meta[pos] = ((uint32_t)act << 8) | (uint32_t)(p.rank & 0xFF);
-            } else {
-              atomicExch(&p.ctr->store_overflow, 1ULL);
-            }
-          }
-        }
-      } else {
-        // route: owner = high bits of the fingerprint scaled to n_ranks (hash-range partition).
-        // A successor whose fingerprint this rank has already routed is known to its owner: drop it
-        // here (direct-mapped, exact-compare cache: misses only cost a redundant record).
-        // (the slot is written only once the record is in the send region: a chunk re-run after a region overflow
-        // must find none of its own dropped records in the cache)
-        unsigned long long* cslot = (has && p.sent_cache) ? p.sent_cache + (fp & p.sent_mask) : nullptr;
-        if (cslot && __ldcv(cslot) == fp) { has = false; cslot = nullptr; }
-        int owner = has ? (int)tlag_owner_k(succ, W, (uint32_t)p.n_ranks, p.owner_words) : -1;
-        const unsigned peers = __match_any_sync(0xffffffffu, owner);
-        if (has) {
-          const int leader = __ffs((int)peers) - 1;
-          unsigned long long base = 0;
-          if ((int)lane == leader) base = atomicAdd(&p.ctr->send_count[owner], (unsigned long long)__popc(peers));
-          base = __shfl_sync(peers, base, leader);
-          const unsigned long long pos = base + (unsigned long long)__popc(peers & lanemask_lt());
-          if (pos < p.region_cap) {
-            uint32_t* dst = p.send + ((unsigned long long)owner * p.region_cap + pos) * (unsigned long long)(W + 2);
-            for (int i = 0; i < W; ++i) dst[i] = succ[i];
-            dst[W] = (uint32_t)idx;
-            dst[W + 1] = ((uint32_t)act << 8) | (uint32_t)(p.rank & 0xFF);
-            if (cslot) *cslot = fp;
-          } else {
-            atomicExch(&p.ctr->route_overflow, 1ULL);
-          }
-        }
+        if (isnew) store_append(p, m, succ, W, (uint32_t)idx, tlag_meta(act, p.rank));
+      } else if (has) {
+        // route: every successor goes to the send region of its owner (tlag_owner_k: hash of its last packed words)
+        route_append(p, succ, W, fp, (int)tlag_owner_k(succ, W, (uint32_t)p.n_ranks, p.owner_words), (uint32_t)idx,
+                     tlag_meta(act, p.rank));
       }
       if (st == L_EMIT) { st = L_RUN; pc = rpc; }
     }
@@ -304,8 +264,8 @@ k_wave(DevParams p, unsigned long long lo, unsigned long long hi) {
 #endif  // !TLAG_SLICED_INC
 
 // ------------------------------------------------------------------ K1 alone: fingerprint + probe/insert
-// One thread per candidate state; W words loaded with the widest aligned vector the layout allows.
-template <int VEC>
+// One thread per candidate state, word by word: the inputs the staged form does not take (W = 1, or a batch that is not
+// 16-byte aligned).
 __global__ void __launch_bounds__(256) k_probe(const uint32_t* __restrict__ states, unsigned long long n, int W,
                                                unsigned long long* table, unsigned long long mask,
                                                uint8_t* __restrict__ is_new, Counters* ctr) {
@@ -313,27 +273,10 @@ __global__ void __launch_bounds__(256) k_probe(const uint32_t* __restrict__ stat
   if (i >= n) return;
   const uint32_t* src = states + i * (unsigned long long)W;
   uint64_t h = tlag_fp_init(W);
-  if (VEC == 4) {
-    const uint4* s4 = reinterpret_cast<const uint4*>(src);
-    const int n4 = W / 4;
-#pragma unroll 5
-    for (int k = 0; k < n4; ++k) {
-      const uint4 v = __ldg(s4 + k);
-      h = tlag_fp_pair(h, v.x, v.y);
-      h = tlag_fp_pair(h, v.z, v.w);
-    }
-  } else if (VEC == 2) {
-    const uint2* s2 = reinterpret_cast<const uint2*>(src);
-    for (int k = 0; k < W / 2; ++k) { const uint2 v = __ldg(s2 + k); h = tlag_fp_pair(h, v.x, v.y); }
-  } else {
-    int k = 0;
-    for (; k + 1 < W; k += 2) h = tlag_fp_pair(h, __ldg(src + k), __ldg(src + k + 1));
-    if (k < W) h = tlag_fp_tail(h, __ldg(src + k));
-  }
-  const unsigned long long fp = tlag_fp_final(h, W);
-  int ins = seen_insert(table, mask, fp);
-  if (ins < 0) { atomicExch(&ctr->table_full, 1ULL); ins = 0; }
-  is_new[i] = (uint8_t)ins;
+  int k = 0;
+  for (; k + 1 < W; k += 2) h = tlag_fp_pair(h, __ldg(src + k), __ldg(src + k + 1));
+  if (k < W) h = tlag_fp_tail(h, __ldg(src + k));
+  is_new[i] = (uint8_t)seen_report(ctr, seen_insert(table, mask, tlag_fp_final(h, W)));
 }
 
 // K1, coalesced form: a CTA of 256 threads owns 256 consecutive candidates = one contiguous span of
@@ -341,13 +284,12 @@ __global__ void __launch_bounds__(256) k_probe(const uint32_t* __restrict__ stat
 // exactly once; ncu on the strided v0 showed 2.4x DRAM read amplification from L1 thrash), staged in
 // shared memory with an odd row stride (W|1 words -> conflict-free), then each thread fingerprints its
 // own row and probes the table.
-#define TLAG_PROBE_ROWS 1   /* rows per thread of the staged form */
 __global__ void __launch_bounds__(256) k_probe_staged(const uint32_t* __restrict__ states, unsigned long long n, int W,
                                                       unsigned long long* table, unsigned long long mask,
                                                       uint8_t* __restrict__ is_new, Counters* ctr) {
   extern __shared__ uint32_t s_rows[];
   const int stride = W | 1;
-  const unsigned ROWS = 256 * TLAG_PROBE_ROWS;
+  const unsigned ROWS = 256;
   const unsigned long long base = (unsigned long long)blockIdx.x * ROWS;
   const unsigned nst = (unsigned)((n - base) < (unsigned long long)ROWS ? (n - base) : (unsigned long long)ROWS);
   const uint32_t* g = states + base * (unsigned long long)W;
@@ -368,178 +310,37 @@ __global__ void __launch_bounds__(256) k_probe_staged(const uint32_t* __restrict
     s_rows[row * stride + col] = g[wi];
   }
   __syncthreads();
-  unsigned long long fp[TLAG_PROBE_ROWS];
-  unsigned long long slot[TLAG_PROBE_ROWS];
-  unsigned long long cur[TLAG_PROBE_ROWS];
-  bool live[TLAG_PROBE_ROWS];
-#pragma unroll
-  for (int q = 0; q < TLAG_PROBE_ROWS; ++q) {
-    const unsigned row = threadIdx.x + 256u * q;
-    live[q] = row < nst;
-    const uint32_t* r = s_rows + (live[q] ? row : 0) * stride;
-    uint64_t h = tlag_fp_init(W);
-    int k = 0;
-    for (; k + 1 < W; k += 2) h = tlag_fp_pair(h, r[k], r[k + 1]);
-    if (k < W) h = tlag_fp_tail(h, r[k]);
-    fp[q] = tlag_fp_final(h, W);
-    slot[q] = fp[q] & mask;
-  }
-  // first probe of every row issued back to back (independent loads in flight), then resolved
-#pragma unroll
-  for (int q = 0; q < TLAG_PROBE_ROWS; ++q) cur[q] = live[q] ? __ldcv(&table[slot[q]]) : 0ULL;
-#pragma unroll
-  for (int q = 0; q < TLAG_PROBE_ROWS; ++q) {
-    if (!live[q]) continue;
-    int ins;
-    if (cur[q] == fp[q]) ins = 0;
-    else if (cur[q] == 0ULL) {
-      const unsigned long long old = atomicCAS(&table[slot[q]], 0ULL, fp[q]);
-      ins = (old == 0ULL) ? 1 : (old == fp[q] ? 0 : seen_insert(table, mask, fp[q]));
-    } else {
-      ins = seen_insert(table, mask, fp[q]);        // collision chain: generic path from the home slot
-    }
-    if (ins < 0) { atomicExch(&ctr->table_full, 1ULL); ins = 0; }
-    is_new[base + threadIdx.x + 256u * q] = (uint8_t)ins;
-  }
+  if (threadIdx.x >= nst) return;
+  const uint32_t* r = s_rows + threadIdx.x * stride;
+  uint64_t h = tlag_fp_init(W);
+  int k = 0;
+  for (; k + 1 < W; k += 2) h = tlag_fp_pair(h, r[k], r[k + 1]);
+  if (k < W) h = tlag_fp_tail(h, r[k]);
+  const unsigned long long fp = tlag_fp_final(h, W);
+  is_new[base + threadIdx.x] = (uint8_t)seen_report(ctr, seen_insert_at(table, mask, fp, __ldcv(&table[fp & mask])));
 }
 
-// K1, TMA form (W a multiple of 4 with W/4 odd: W = 4, 12, 20 ...).  A persistent CTA streams its tiles of
-// 512 rows through a 2-stage shared-memory ring filled by 1-D bulk copies of the TMA engine (cp.async.bulk ...
-// mbarrier::complete_tx::bytes -- UBLKCP in SASS): one elected thread arms the stage's mbarrier with the byte count and
-// issues the copy, the copy of tile k+1 is in flight while tile k is hashed and probed, and no thread spends issue
-// slots on LDG -> STS staging.  Rows are dense in shared memory (pitch = 4 W bytes, no padding) and read back with
-// 128-bit LDS: for W/4 odd the 8 rows of a quarter-warp fall into 8 distinct 4-bank groups, so the loads are
-// conflict-free.  Every thread owns TWO rows per tile: both fingerprints are computed first, both home-slot loads are
-// issued back to back (two independent DRAM round trips in flight per thread), then resolved.
-#define TLAG_TMA_ROWS 2
-#define TLAG_TMA_STAGES 2
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint64_t* b, unsigned count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(b)), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* b, unsigned bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(b)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void bulk_g2s(void* dst, const void* src, unsigned bytes, uint64_t* b) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-               ::"r"(smem_u32(dst)), "l"(src), "r"(bytes), "r"(smem_u32(b)) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* b, unsigned parity) {
-  unsigned ok;
-  do {
-    asm volatile("{ .reg .pred p; mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2; selp.u32 %0, 1, 0, p; }"
-                 : "=r"(ok) : "r"(smem_u32(b)), "r"(parity) : "memory");
-  } while (!ok);
+// One routed record (W state words, parent, meta) into this rank's shard: fingerprint, probe, append.  Every lane of the
+// warp calls it; `has` says whether the lane holds a record.  Read through L2: the inbox of k_insert_inbox is written by
+// peers over NVLink.
+__device__ __forceinline__ void insert_record(const DevParams& p, const uint32_t* rec, bool has) {
+  const int W = p.W;
+  uint32_t w[TLAG_MAXW];
+  unsigned long long fp = 0;
+  if (has) {
+    for (int k = 0; k < W; ++k) w[k] = __ldcg(rec + k);
+    fp = tlag_fingerprint(w, W);
+  }
+  const bool isnew = has && seen_report(p.ctr, seen_insert(p.table, p.mask, fp));
+  const unsigned m = __ballot_sync(0xffffffffu, isnew);
+  if (isnew) store_append(p, m, w, W, __ldcg(rec + W), __ldcg(rec + W + 1));
 }
 
-__global__ void __launch_bounds__(256) k_probe_tma(const uint32_t* __restrict__ states, unsigned long long n, int W,
-                                                   unsigned long long* table, unsigned long long mask,
-                                                   uint8_t* __restrict__ is_new, Counters* ctr) {
-  extern __shared__ __align__(128) uint8_t s_ring[];
-  __shared__ __align__(8) uint64_t s_full[TLAG_TMA_STAGES];
-  constexpr unsigned ROWS = 256 * TLAG_TMA_ROWS;
-  const unsigned row_bytes = (unsigned)W * 4u;
-  const unsigned tile_bytes = ROWS * row_bytes;
-  const unsigned long long n_tiles = (n + ROWS - 1) / ROWS;
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < TLAG_TMA_STAGES; ++s) mbar_init(&s_full[s], 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  __syncthreads();
-  auto issue = [&](unsigned long long tile, int stage) {
-    const unsigned long long first = tile * ROWS;
-    const unsigned rows = (unsigned)((n - first) < (unsigned long long)ROWS ? (n - first) : (unsigned long long)ROWS);
-    const unsigned bytes = rows * row_bytes;
-    mbar_expect_tx(&s_full[stage], bytes);
-    bulk_g2s(s_ring + (size_t)stage * tile_bytes, states + first * (unsigned long long)W, bytes, &s_full[stage]);
-  };
-  if (threadIdx.x == 0)
-    for (int s = 0; s < TLAG_TMA_STAGES; ++s) {
-      const unsigned long long t = blockIdx.x + (unsigned long long)s * gridDim.x;
-      if (t < n_tiles) issue(t, s);
-    }
-  unsigned long long k = 0;
-  for (unsigned long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++k) {
-    const int stage = (int)(k % TLAG_TMA_STAGES);
-    mbar_wait(&s_full[stage], (unsigned)((k / TLAG_TMA_STAGES) & 1));
-    const unsigned long long first = tile * ROWS;
-    const unsigned nst = (unsigned)((n - first) < (unsigned long long)ROWS ? (n - first) : (unsigned long long)ROWS);
-    const uint8_t* base = s_ring + (size_t)stage * tile_bytes;
-    unsigned long long fp[TLAG_TMA_ROWS], slot[TLAG_TMA_ROWS], cur[TLAG_TMA_ROWS];
-    bool live[TLAG_TMA_ROWS];
-#pragma unroll
-    for (int q = 0; q < TLAG_TMA_ROWS; ++q) {
-      const unsigned row = threadIdx.x + 256u * q;
-      live[q] = row < nst;
-      const uint4* r4 = reinterpret_cast<const uint4*>(base + (size_t)(live[q] ? row : 0) * row_bytes);
-      uint64_t h = tlag_fp_init(W);
-      for (int j = 0; j < W / 4; ++j) {
-        const uint4 v = r4[j];
-        h = tlag_fp_pair(h, v.x, v.y);
-        h = tlag_fp_pair(h, v.z, v.w);
-      }
-      fp[q] = tlag_fp_final(h, W);
-      slot[q] = fp[q] & mask;
-    }
-#pragma unroll
-    for (int q = 0; q < TLAG_TMA_ROWS; ++q) cur[q] = live[q] ? __ldcv(&table[slot[q]]) : 0ULL;
-    __syncthreads();                                   // every row of this stage has been read: refill it
-    if (threadIdx.x == 0) {
-      const unsigned long long nt = tile + (unsigned long long)TLAG_TMA_STAGES * gridDim.x;
-      if (nt < n_tiles) issue(nt, stage);
-    }
-#pragma unroll
-    for (int q = 0; q < TLAG_TMA_ROWS; ++q) {
-      if (!live[q]) continue;
-      int ins;
-      if (cur[q] == fp[q]) ins = 0;
-      else if (cur[q] == 0ULL) {
-        const unsigned long long old = atomicCAS(&table[slot[q]], 0ULL, fp[q]);
-        ins = (old == 0ULL) ? 1 : (old == fp[q] ? 0 : seen_insert(table, mask, fp[q]));
-      } else {
-        ins = seen_insert(table, mask, fp[q]);
-      }
-      if (ins < 0) { atomicExch(&ctr->table_full, 1ULL); ins = 0; }
-      is_new[first + threadIdx.x + 256u * q] = (uint8_t)ins;
-    }
-  }
-}
-
-// insert routed records (W state words + parent + meta) into this rank's shard
+// insert routed records into this rank's shard
 __global__ void __launch_bounds__(256) k_insert_records(DevParams p, const uint32_t* __restrict__ rec,
                                                         unsigned long long n) {
   const unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
-  const unsigned lane = threadIdx.x & 31;
-  const int W = p.W;
-  uint32_t w[TLAG_MAXW];
-  bool has = i < n;
-  unsigned long long fp = 0;
-  const uint32_t* src = rec + i * (unsigned long long)(W + 2);
-  if (has) {
-    for (int k = 0; k < W; ++k) w[k] = src[k];
-    fp = tlag_fingerprint(w, W);
-  }
-  int ins = has ? seen_insert(p.table, p.mask, fp) : 0;
-  if (ins < 0) { atomicExch(&p.ctr->table_full, 1ULL); ins = 0; }
-  const bool isnew = ins > 0;
-  const unsigned m = __ballot_sync(0xffffffffu, isnew);
-  if (m) {
-    const int leader = __ffs((int)m) - 1;
-    unsigned long long base = 0;
-    if ((int)lane == leader) base = atomicAdd(&p.ctr->n_states, (unsigned long long)__popc(m));
-    base = __shfl_sync(0xffffffffu, base, leader);
-    if (isnew) {
-      const unsigned long long pos = base + (unsigned long long)__popc(m & lanemask_lt());
-      if (pos < p.cap_states) {
-        uint32_t* dst = p.states + pos * (unsigned long long)W;
-        for (int k = 0; k < W; ++k) dst[k] = w[k];
-        p.parent[pos] = src[W];
-        p.meta[pos] = src[W + 1];
-      } else {
-        atomicExch(&p.ctr->store_overflow, 1ULL);
-      }
-    }
-  }
+  insert_record(p, rec + i * (unsigned long long)(p.W + 2), i < n);
 }
 
 // ------------------------------------------------------------------ peer-memory exchange (multi-GPU)
@@ -592,8 +393,6 @@ __global__ void __launch_bounds__(256) k_push(P2PParams q, const Counters* ctr, 
 
 // Inserts every source's records of chunk `seq` (grid-stride over sources and records, whole warps).
 __global__ void __launch_bounds__(256) k_insert_inbox(DevParams p, P2PParams q, unsigned long long seq) {
-  const unsigned lane = threadIdx.x & 31;
-  const int W = p.W;
   __shared__ unsigned long long s_n;
   __shared__ int s_last;
   for (int src = 0; src < q.n_ranks; ++src) {
@@ -607,37 +406,8 @@ __global__ void __launch_bounds__(256) k_insert_inbox(DevParams p, P2PParams q, 
     const uint32_t* rec = q.inbox + (((seq & 1ULL) * q.n_ranks + src) * q.inbox_cap) * q.rec_words;
     const unsigned long long n32 = (n + 31ULL) & ~31ULL;
     for (unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; i < n32;
-         i += (unsigned long long)gridDim.x * blockDim.x) {
-      uint32_t w[TLAG_MAXW];
-      const bool has = i < n;
-      unsigned long long fp = 0;
-      const uint32_t* r = rec + i * (unsigned long long)(W + 2);
-      if (has) {
-        for (int k = 0; k < W; ++k) w[k] = __ldcg(r + k);      // written by a peer over NVLink: read through L2
-        fp = tlag_fingerprint(w, W);
-      }
-      int ins = has ? seen_insert(p.table, p.mask, fp) : 0;
-      if (ins < 0) { atomicExch(&p.ctr->table_full, 1ULL); ins = 0; }
-      const bool isnew = ins > 0;
-      const unsigned mk = __ballot_sync(0xffffffffu, isnew);
-      if (mk) {
-        const int leader = __ffs((int)mk) - 1;
-        unsigned long long base = 0;
-        if ((int)lane == leader) base = atomicAdd(&p.ctr->n_states, (unsigned long long)__popc(mk));
-        base = __shfl_sync(0xffffffffu, base, leader);
-        if (isnew) {
-          const unsigned long long pos = base + (unsigned long long)__popc(mk & lanemask_lt());
-          if (pos < p.cap_states) {
-            uint32_t* dst = p.states + pos * (unsigned long long)W;
-            for (int k = 0; k < W; ++k) dst[k] = w[k];
-            p.parent[pos] = __ldcg(r + W);
-            p.meta[pos] = __ldcg(r + W + 1);
-          } else {
-            atomicExch(&p.ctr->store_overflow, 1ULL);
-          }
-        }
-      }
-    }
+         i += (unsigned long long)gridDim.x * blockDim.x)
+      insert_record(p, rec + i * (unsigned long long)(p.W + 2), i < n);
     __syncthreads();
   }
   // every block is done with every source: the last one acknowledges the chunk to all sources
@@ -947,6 +717,26 @@ static int cluster_slice(tlag_engine* e, uint64_t first, uint64_t count) {
   return TLAG_OK;
 }
 
+// the counters of a search that has discovered nothing: zero, and the violation slots (minimum keys) at "none"
+static int reset_counters(tlag_engine* e) {
+  Counters hc;
+  memset(&hc, 0, sizeof(hc));
+  hc.viol_inv = hc.viol_assert = hc.viol_trap = hc.viol_deadlock = ~0ULL;
+  CK(cudaMemcpyAsync(e->d_ctr, &hc, sizeof(hc), cudaMemcpyHostToDevice, e->stream));   // pageable: staged before return
+  return TLAG_OK;
+}
+
+// Route mode with several ranks: the direct-mapped cache of the fingerprints this rank has routed (2^26 x 8 B = 512 MB).
+// It is only a filter: without memory for it, or with TLAG_NO_SENT_CACHE set, every successor is routed.
+static int ensure_sent_cache(tlag_engine* e) {
+  if (e->d_sent || e->p.n_ranks < 2 || getenv("TLAG_NO_SENT_CACHE") != nullptr) return TLAG_OK;
+  const unsigned long long slots = 1ULL << 26;
+  if (dmalloc(e, &e->d_sent, slots * 8) != cudaSuccess) { cudaGetLastError(); e->d_sent = nullptr; return TLAG_OK; }
+  CK(cudaMemsetAsync(e->d_sent, 0, slots * 8, e->stream));
+  e->p.sent_cache = e->d_sent; e->p.sent_mask = slots - 1;
+  return TLAG_OK;
+}
+
 #if defined(TLAG_SLICED_INC)
 extern "C" const char* tlag_version(void) { return "tlag 0.2 (sm_90a) native sliced"; }
 #else
@@ -1012,10 +802,8 @@ extern "C" int tlag_create(const tlag_model* m, tlag_engine** out) {
   CK(cudaMalloc(&e->d_layout, (size_t)(m->n_slots ? m->n_slots : 1) * sizeof(tlag_slot)));
   CK(cudaMemcpy(e->d_layout, m->layout, (size_t)m->n_slots * sizeof(tlag_slot), cudaMemcpyHostToDevice));
   CK(cudaMalloc(&e->d_ctr, sizeof(Counters)));
-  Counters hc;
-  memset(&hc, 0, sizeof(hc));
-  hc.viol_inv = hc.viol_assert = hc.viol_trap = hc.viol_deadlock = ~0ULL;
-  CK(cudaMemcpy(e->d_ctr, &hc, sizeof(hc), cudaMemcpyHostToDevice));
+  int r = reset_counters(e);
+  if (r) return r;
   // state store
   uint64_t cap = m->max_states ? m->max_states : (1ULL << 20);
   if (cap < 1024) cap = 1024;
@@ -1058,7 +846,7 @@ extern "C" int tlag_create(const tlag_model* m, tlag_engine** out) {
     e->p.stage = (s_ && *s_) ? (atoi(s_) > 0 ? atoi(s_) : 0) : INT_MAX;
   }
   unsigned log2 = m->table_slots_log2 ? m->table_slots_log2 : 22;
-  int r = alloc_table(e, log2);
+  r = alloc_table(e, log2);
   if (r) return r;
   CK(cudaStreamSynchronize(e->stream));
   return TLAG_OK;
@@ -1101,28 +889,13 @@ static int launch_probe(tlag_engine* e, const uint32_t* d_states, uint64_t n, ui
   const int W = (int)e->m.words_per_state;
   const unsigned blocks = (unsigned)((n + 255) / 256);
   if (n == 0) return TLAG_OK;
-  const bool a16 = ((uintptr_t)d_states % 16) == 0, a8 = ((uintptr_t)d_states % 8) == 0;
-  // TLAG_K1_TMA=1 selects the TMA-ring form.  The staged form is the default: the ring's shared memory (2 x 40 KB per
-  // CTA at W = 20) halves the resident threads, and K1 is bound by the latency of the random table probes, not by the
-  // row copies the TMA engine takes over.
-  static const bool use_tma = getenv("TLAG_K1_TMA") != nullptr;
-  if (a16 && W % 4 == 0 && ((W / 4) & 1) && use_tma) {
-    const size_t smem = (size_t)TLAG_TMA_STAGES * 256 * TLAG_TMA_ROWS * (size_t)W * 4;
-    CK(cudaFuncSetAttribute(k_probe_tma, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    int occ = 1;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_probe_tma, 256, smem) != cudaSuccess || occ < 1) occ = 1;
-    const uint64_t tiles = (n + 256 * TLAG_TMA_ROWS - 1) / (256 * TLAG_TMA_ROWS);
-    uint64_t grid = (uint64_t)e->sm_count * (uint64_t)occ;                // persistent: one resident wave of CTAs
-    if (grid > tiles) grid = tiles;
-    k_probe_tma<<<(unsigned)grid, 256, smem, e->stream>>>(d_states, n, W, e->d_table, e->p.mask, d_is_new, e->d_ctr);
-  } else if (a16 && W >= 2) {
-    const size_t smem = (size_t)256 * TLAG_PROBE_ROWS * (size_t)(W | 1) * 4;
+  if (((uintptr_t)d_states % 16) == 0 && W >= 2) {
+    const size_t smem = (size_t)256 * (size_t)(W | 1) * 4;
     if (smem > 48 * 1024) CK(cudaFuncSetAttribute(k_probe_staged, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    const unsigned sblocks = (unsigned)((n + 256 * TLAG_PROBE_ROWS - 1) / (256 * TLAG_PROBE_ROWS));
-    k_probe_staged<<<sblocks, 256, smem, e->stream>>>(d_states, n, W, e->d_table, e->p.mask, d_is_new, e->d_ctr);
-  } else if (W % 4 == 0 && a16) k_probe<4><<<blocks, 256, 0, e->stream>>>(d_states, n, W, e->d_table, e->p.mask, d_is_new, e->d_ctr);
-  else if (W % 2 == 0 && a8) k_probe<2><<<blocks, 256, 0, e->stream>>>(d_states, n, W, e->d_table, e->p.mask, d_is_new, e->d_ctr);
-  else k_probe<1><<<blocks, 256, 0, e->stream>>>(d_states, n, W, e->d_table, e->p.mask, d_is_new, e->d_ctr);
+    k_probe_staged<<<blocks, 256, smem, e->stream>>>(d_states, n, W, e->d_table, e->p.mask, d_is_new, e->d_ctr);
+  } else {
+    k_probe<<<blocks, 256, 0, e->stream>>>(d_states, n, W, e->d_table, e->p.mask, d_is_new, e->d_ctr);
+  }
   e->launches++;
   CK(cudaGetLastError());
   return TLAG_OK;
@@ -1212,10 +985,8 @@ extern "C" int tlag_seed(tlag_engine* e, const uint32_t* states, uint64_t n) {
 // Forget everything discovered and start again from the retained initial states (bench loops).
 extern "C" int tlag_restart(tlag_engine* e) {
   if (!e) return TLAG_EINVAL;
-  Counters hc;
-  memset(&hc, 0, sizeof(hc));
-  hc.viol_inv = hc.viol_assert = hc.viol_trap = hc.viol_deadlock = ~0ULL;
-  CK(cudaMemcpyAsync(e->d_ctr, &hc, sizeof(hc), cudaMemcpyHostToDevice, e->stream));
+  int r = reset_counters(e);
+  if (r) return r;
   CK(cudaMemsetAsync(e->d_table, 0, (1ULL << e->table_log2) * 8, e->stream));
   if (e->d_sent) CK(cudaMemsetAsync(e->d_sent, 0, (e->p.sent_mask + 1) * 8, e->stream));
   CK(cudaStreamSynchronize(e->stream));
@@ -1224,7 +995,7 @@ extern "C" int tlag_restart(tlag_engine* e) {
   e->kg_verdict = 0;
   e->restarting = true;
   const uint64_t W = e->m.words_per_state;
-  int r = tlag_seed(e, e->h_init.data(), e->h_init.size() / W);
+  r = tlag_seed(e, e->h_init.data(), e->h_init.size() / W);
   e->restarting = false;
   return r;
 }
@@ -1499,13 +1270,8 @@ extern "C" int tlag_expand_route(tlag_engine* e, uint32_t n_ranks, uint64_t firs
     if (n_ranks > 1) { e->err = "tlag_expand_route: call tlag_set_rank(n_ranks, rank) first"; return TLAG_ESTATE; }
     e->p.n_ranks = 1; e->p.rank = 0;
   }
-  if (!e->d_sent && n_ranks > 1 && getenv("TLAG_NO_SENT_CACHE") == nullptr) {
-    const unsigned lg = 26;                                    // 2^26 x 8 B = 512 MB
-    if (dmalloc(e, &e->d_sent, (1ULL << lg) * 8) == cudaSuccess) {
-      CK(cudaMemsetAsync(e->d_sent, 0, (1ULL << lg) * 8, e->stream));
-      e->p.sent_cache = e->d_sent; e->p.sent_mask = (1ULL << lg) - 1;
-    } else { cudaGetLastError(); e->d_sent = nullptr; }
-  }
+  int r = ensure_sent_cache(e);
+  if (r) return r;
   e->p.send = (uint32_t*)(uintptr_t)d_send;
   e->p.region_cap = cap_records / n_ranks;
   CK(cudaMemsetAsync(&e->d_ctr->work, 0, 8, e->stream));
@@ -1583,36 +1349,22 @@ extern "C" int tlag_p2p_init(tlag_engine* e, uint32_t n_ranks, uint32_t rank, ui
   static_assert(sizeof(cudaIpcMemHandle_t) == 64, "IPC handle size");
   const uint64_t rw = e->m.words_per_state + 2;
   cap_records = (cap_records + 3) & ~3ULL;                       // regions stay 16-byte aligned
-  for (size_t i = 0; i < g_p2p_parked.size(); ++i) {
+  for (size_t i = 0; i < g_p2p_parked.size() && e->p2p_slot < 0; ++i) {
     P2PParked& c = g_p2p_parked[i];
     if (c.in_use || c.device != e->m.device || c.n_ranks != (int)n_ranks || c.rank != (int)rank || c.rec_words != (int)rw ||
         c.cap != cap_records) continue;
     c.in_use = true;
     e->p2p_slot = (int)i;
     e->d_p2p = c.d_p2p; e->p2p_bytes = c.bytes; e->d_send_own = c.d_send; e->d_tickets = c.d_tickets; e->p2p_seq = c.seq;
-    memset(&e->q, 0, sizeof(e->q));
-    e->q.n_ranks = (int)n_ranks; e->q.rank = (int)rank; e->q.rec_words = (int)rw;
-    e->q.inbox_cap = cap_records; e->q.region_cap = cap_records;
-    e->q.send = e->d_send_own;
-    e->q.meta = (P2PMeta*)e->d_p2p;
-    e->q.inbox = (uint32_t*)((uint8_t*)e->d_p2p + p2p_meta_bytes());
-    e->q.tickets = e->d_tickets;
-    e->peer_base[rank] = e->d_p2p;
-    e->q.peer_meta[rank] = e->q.meta; e->q.peer_inbox[rank] = e->q.inbox;
-    cudaIpcMemHandle_t h;
-    CK(cudaIpcGetMemHandle(&h, e->d_p2p));
-    memcpy(handle_out64, &h, 64);
-    e->p.n_ranks = (int)n_ranks; e->p.rank = (int)rank;
-    return TLAG_OK;
   }
-  const uint64_t inbox_bytes = 2ULL * n_ranks * cap_records * rw * 4;
-  e->p2p_bytes = p2p_meta_bytes() + inbox_bytes;
-  CK(cudaMalloc(&e->d_p2p, e->p2p_bytes));
-  CK(cudaMemset(e->d_p2p, 0, p2p_meta_bytes()));
-  CK(cudaMalloc(&e->d_send_own, (uint64_t)n_ranks * cap_records * rw * 4));
-  CK(cudaMalloc(&e->d_tickets, 32 * sizeof(unsigned int)));
-  CK(cudaMemset(e->d_tickets, 0, 32 * sizeof(unsigned int)));
-  {
+  if (e->p2p_slot < 0) {
+    const uint64_t inbox_bytes = 2ULL * n_ranks * cap_records * rw * 4;
+    e->p2p_bytes = p2p_meta_bytes() + inbox_bytes;
+    CK(cudaMalloc(&e->d_p2p, e->p2p_bytes));
+    CK(cudaMemset(e->d_p2p, 0, p2p_meta_bytes()));
+    CK(cudaMalloc(&e->d_send_own, (uint64_t)n_ranks * cap_records * rw * 4));
+    CK(cudaMalloc(&e->d_tickets, 32 * sizeof(unsigned int)));
+    CK(cudaMemset(e->d_tickets, 0, 32 * sizeof(unsigned int)));
     P2PParked c;
     memset(&c, 0, sizeof(c));
     c.device = e->m.device; c.n_ranks = (int)n_ranks; c.rank = (int)rank; c.rec_words = (int)rw; c.cap = cap_records;
@@ -1682,13 +1434,8 @@ extern "C" int tlag_p2p_level(tlag_engine* e, uint64_t n_chunks, uint64_t chunk_
   r = grow_table_if_needed(e, before + expect);
   if (r) return r;
   e->p.n_ranks = (int)n_ranks; e->p.rank = e->q.rank;
-  if (!e->d_sent && n_ranks > 1 && getenv("TLAG_NO_SENT_CACHE") == nullptr) {
-    const unsigned lg = 26;                                    // 2^26 x 8 B = 512 MB
-    if (dmalloc(e, &e->d_sent, (1ULL << lg) * 8) == cudaSuccess) {
-      CK(cudaMemsetAsync(e->d_sent, 0, (1ULL << lg) * 8, e->stream));
-      e->p.sent_cache = e->d_sent; e->p.sent_mask = (1ULL << lg) - 1;
-    } else { cudaGetLastError(); e->d_sent = nullptr; }
-  }
+  r = ensure_sent_cache(e);
+  if (r) return r;
   e->p.send = e->d_send_own;
   e->p.region_cap = e->q.region_cap;
   CK(cudaMemsetAsync(&e->d_ctr->route_overflow, 0, 8, e->stream));
