@@ -70,6 +70,7 @@ typedef struct {
   uint64_t generated_total;
   float    kernel_ms;            /* device time of the wave kernel (CUDA events)               */
   int32_t  verdict;              /* TLAG_V_RUNNING while the search continues                  */
+  float    cluster_ms;           /* device time of the level's frontier clustering pass (events) */
 } tlag_wave_stats;
 
 typedef struct {

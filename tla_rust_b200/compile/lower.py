@@ -4479,7 +4479,7 @@ class Lowering:
 
     def _cluster_slots_last(self, lay):
         """Pack order for models with containers.  The engine clusters each BFS level, and partitions the state
-        space over GPUs, by the LAST TWO packed words (tlag_owner, k_sort_keys).  With containers laid out in
+        space over GPUs, by the LAST TWO packed words (tlag_owner, the frontier clustering key).  With containers laid out in
         variable order those words would hold the zero tail of the last container (no entropy: every state on one
         rank).  So the "control" slots -- scalar variables, elements of small per-process functions, container
         lengths, presence flags -- are packed last, up to 64 bits of them."""

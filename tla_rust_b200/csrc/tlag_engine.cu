@@ -75,6 +75,8 @@ struct tlag_engine {
   bool restarting = false;
   double growth_hint = 4.0;
   void* d_sort = nullptr; uint64_t sort_bytes = 0;
+  // clustering pass: the rank set ([RankSetCtl | 2^log2 keys | 2^log2 ranks]), its size carried from level to level
+  void* d_rset = nullptr; uint64_t rset_bytes = 0; unsigned rset_log2 = 16; bool rset_fixed = false;
   unsigned long long* d_sent = nullptr;
   uint8_t* d_succ = nullptr; uint64_t succ_cap = 0;   // sliced build: per-frontier-state "has a successor" flags
   unsigned long long* d_dig = nullptr;                // tlag_digest accumulators (XOR, SUM)
@@ -441,27 +443,154 @@ __global__ void k_digest(DevParams p, unsigned long long n, unsigned long long* 
 // variables, for the Paxos models the high bits of the msgs bitset) follow similar paths: measured on
 // a 4096-state window of MCPaxos3_b3 level 14, lane utilisation is 0.35 in discovery order, 0.31 in random
 // order and 0.54 when sorted by the last packed word.  Each newly discovered level slice is therefore
-// reordered (stable data: nothing references those indices yet) by a 64-bit key of its last two words.
-__global__ void k_sort_keys(const uint32_t* __restrict__ states, unsigned long long n, int W,
-                            unsigned long long* __restrict__ keys, uint32_t* __restrict__ idx) {
+// reordered (stable data: nothing references those indices yet) by a 64-bit key of its last two words,
+// key = w[W-1] << 32 | w[W-2], stably, so equal keys keep their discovery order.
+//
+// A level holds few distinct keys (MCPaxos3_b4: 1 K - 100 K in levels of up to millions of states; Raft and SSI a few
+// hundred), so the slice is sorted on the key's dense rank among the level's distinct keys, not on the key itself: the
+// same permutation, on 32-bit keys of ceil(log2(distinct)) bits -- 2 or 3 radix passes instead of 8 passes over 64-bit
+// keys.  The pass:
+//   k_cluster_pack    copies the slice's rows, parents and meta words out of the store into records of W + 2 words
+//                     (one contiguous read per record later) and writes each state's key;
+//   k_rset_insert     puts the keys into a small open-addressed set (the rank set, L2-resident at these sizes);
+//   k_rset_list, a sort of the distinct keys, k_rset_rank   give every distinct key its rank;
+//   k_rank_states     writes each state's rank, then a stable radix sort of (rank, index) over the rank's bits;
+//   k_cluster_gather  writes record idx[i] to store row first + i, a warp per 32 rows, stores coalesced.
+#define TLAG_RSET_EMPTY 0xFFFFFFFFFFFFFFFFull   /* empty slot; a key equal to it is counted aside (it is the largest) */
+struct RankSetCtl { unsigned n, full, has_max, n_list; };
+#define TLAG_CLUSTER_ILP 4   /* words each lane loads before it stores them (pack, gather): latency-bound otherwise */
+
+__device__ __forceinline__ unsigned long long rset_hash(unsigned long long k) {   // splitmix64 finaliser
+  k ^= k >> 30; k *= 0xbf58476d1ce4e5b9ull; k ^= k >> 27; k *= 0x94d049bb133111ebull; return k ^ (k >> 31);
+}
+
+__global__ void k_cluster_pack(const uint32_t* __restrict__ st, const uint32_t* __restrict__ parent,
+                               const uint32_t* __restrict__ meta, unsigned long long n, int W,
+                               uint32_t* __restrict__ rec, unsigned long long* __restrict__ keys) {
+  const unsigned lane = threadIdx.x & 31;
+  const unsigned long long r0 = ((unsigned long long)blockIdx.x * blockDim.x + threadIdx.x) & ~31ull;
+  if (r0 >= n) return;
+  const unsigned rows = n - r0 < 32 ? (unsigned)(n - r0) : 32u;
+  const uint32_t* src = st + r0 * (unsigned long long)W;
+  uint32_t* dst = rec + r0 * (unsigned long long)(W + 2);
+  const unsigned long long i = r0 + lane;
+  const uint32_t par = lane < rows ? __ldcs(parent + i) : 0, met = lane < rows ? __ldcs(meta + i) : 0;
+  const unsigned words = rows * (unsigned)W;
+  for (unsigned base = 0; base < words; base += 32 * TLAG_CLUSTER_ILP) {   // several loads in flight per lane
+    uint32_t v[TLAG_CLUSTER_ILP];
+#pragma unroll
+    for (int u = 0; u < TLAG_CLUSTER_ILP; ++u) {
+      const unsigned k = base + u * 32 + lane;
+      v[u] = k < words ? src[k] : 0;
+    }
+#pragma unroll
+    for (int u = 0; u < TLAG_CLUSTER_ILP; ++u) {
+      const unsigned k = base + u * 32 + lane, r = k / (unsigned)W, c = k - r * (unsigned)W;
+      if (k < words) dst[r * (W + 2) + c] = v[u];
+    }
+  }
+  if (lane < rows) {
+    dst[lane * (W + 2) + W] = par;
+    dst[lane * (W + 2) + W + 1] = met;
+    const uint32_t* s = src + lane * (unsigned long long)W;
+    const unsigned long long hi = s[W - 1], lo = W >= 2 ? s[W - 2] : 0;
+    keys[i] = (hi << 32) | lo;
+  }
+}
+
+__global__ void k_rset_insert(const unsigned long long* __restrict__ keys, unsigned long long n,
+                              unsigned long long* __restrict__ table, unsigned long long mask, RankSetCtl* ctl) {
   const unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  const uint32_t* s = states + i * (unsigned long long)W;
-  const unsigned long long hi = s[W - 1], lo = W >= 2 ? s[W - 2] : 0;
-  keys[i] = (hi << 32) | lo;
+  const unsigned long long key = __ldcs(keys + i);
+  // lanes of a warp often share a key (successors of like states): one lane per distinct key probes the set
+  const unsigned peers = __match_any_sync(__activemask(), key);
+  if ((threadIdx.x & 31) != (unsigned)(__ffs(peers) - 1)) return;
+  if (key == TLAG_RSET_EMPTY) { if (!*(volatile unsigned*)&ctl->has_max) ctl->has_max = 1; return; }
+  unsigned long long h = rset_hash(key) & mask;
+  for (unsigned long long probes = 0; probes <= mask; ++probes, h = (h + 1) & mask) {
+    unsigned long long v = __ldcg(table + h);
+    if (v == key) return;
+    if (v == TLAG_RSET_EMPTY) {
+      if (*(volatile unsigned*)&ctl->full) return;
+      v = atomicCAS(table + h, TLAG_RSET_EMPTY, key);
+      if (v == TLAG_RSET_EMPTY) {                 // new distinct key; past half the slots the set is grown and refilled
+        if ((unsigned long long)atomicAdd(&ctl->n, 1u) + 1 > (mask + 1) / 2) ctl->full = 1;
+        return;
+      }
+      if (v == key) return;
+    }
+  }
+  ctl->full = 1;
+}
+
+__global__ void k_rset_list(const unsigned long long* __restrict__ table, unsigned long long slots,
+                            unsigned long long* __restrict__ list, RankSetCtl* ctl) {
+  const unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= slots) return;
+  const unsigned long long v = table[i];
+  if (v != TLAG_RSET_EMPTY) list[atomicAdd(&ctl->n_list, 1u)] = v;
+}
+
+__device__ __forceinline__ unsigned long long rset_find(const unsigned long long* __restrict__ table,
+                                                        unsigned long long mask, unsigned long long key) {
+  unsigned long long h = rset_hash(key) & mask;
+  while (table[h] != key) h = (h + 1) & mask;     // every key looked up was inserted
+  return h;
+}
+
+// sorted[r] = the distinct key of rank r
+__global__ void k_rset_rank(const unsigned long long* __restrict__ sorted, unsigned n,
+                            const unsigned long long* __restrict__ table, unsigned long long mask, uint32_t* __restrict__ rank) {
+  const unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) rank[rset_find(table, mask, sorted[i])] = i;
+}
+
+__global__ void k_rank_states(const unsigned long long* __restrict__ keys, unsigned long long n,
+                              const unsigned long long* __restrict__ table, unsigned long long mask,
+                              const uint32_t* __restrict__ rank, uint32_t max_rank,
+                              uint32_t* __restrict__ r_out, uint32_t* __restrict__ idx) {
+  const unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const unsigned long long key = __ldcs(keys + i);
+  const unsigned peers = __match_any_sync(__activemask(), key);    // one lookup per distinct key of the warp
+  const int leader = __ffs(peers) - 1;
+  uint32_t rk = 0;
+  if ((int)(threadIdx.x & 31) == leader) rk = key == TLAG_RSET_EMPTY ? max_rank : rank[rset_find(table, mask, key)];
+  r_out[i] = __shfl_sync(peers, rk, leader);
   idx[i] = (uint32_t)i;
 }
 
-__global__ void k_gather_slice(const uint32_t* __restrict__ states, const uint32_t* __restrict__ parent,
-                               const uint32_t* __restrict__ meta, const uint32_t* __restrict__ idx,
-                               unsigned long long n, int W, uint32_t* __restrict__ o_states,
-                               uint32_t* __restrict__ o_parent, uint32_t* __restrict__ o_meta) {
-  const unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  const unsigned long long j = idx[i];
-  for (int k = 0; k < W; ++k) o_states[i * (unsigned long long)W + k] = states[j * (unsigned long long)W + k];
-  o_parent[i] = parent[j];
-  o_meta[i] = meta[j];
+__global__ void k_cluster_gather(const uint32_t* __restrict__ rec, const uint32_t* __restrict__ idx,
+                                 unsigned long long n, int W, uint32_t* __restrict__ st,
+                                 uint32_t* __restrict__ parent, uint32_t* __restrict__ meta) {
+  const unsigned lane = threadIdx.x & 31;
+  const unsigned long long r0 = ((unsigned long long)blockIdx.x * blockDim.x + threadIdx.x) & ~31ull;
+  if (r0 >= n) return;
+  const unsigned rows = n - r0 < 32 ? (unsigned)(n - r0) : 32u;
+  const unsigned long long j = lane < rows ? __ldcs(idx + r0 + lane) : 0;
+  const uint32_t* mine = rec + j * (unsigned long long)(W + 2);
+  const uint32_t par = lane < rows ? mine[W] : 0, met = lane < rows ? mine[W + 1] : 0;
+  uint32_t* dst = st + r0 * (unsigned long long)W;
+  const unsigned words = rows * (unsigned)W;
+  for (unsigned base = 0; base < words; base += 32 * TLAG_CLUSTER_ILP) {   // warp-uniform trip count: the shuffle has every lane
+    uint32_t v[TLAG_CLUSTER_ILP];
+#pragma unroll
+    for (int u = 0; u < TLAG_CLUSTER_ILP; ++u) {
+      const unsigned k = base + u * 32 + lane, r = k / (unsigned)W, c = k - r * (unsigned)W;
+      const unsigned long long jr = __shfl_sync(0xffffffffu, j, r & 31);
+      v[u] = k < words ? rec[jr * (unsigned long long)(W + 2) + c] : 0;
+    }
+#pragma unroll
+    for (int u = 0; u < TLAG_CLUSTER_ILP; ++u) {
+      const unsigned k = base + u * 32 + lane;
+      if (k < words) dst[k] = v[u];
+    }
+  }
+  if (lane < rows) {
+    parent[r0 + lane] = par;
+    meta[r0 + lane] = met;
+  }
 }
 
 // rebuild the table from the state store after growing it
@@ -670,50 +799,116 @@ static int grow_store_if_needed(tlag_engine* e, uint64_t need) {
   return TLAG_OK;
 }
 
+// Grows a clustering buffer to at least `bytes` (geometrically when `slack`: levels grow, a re-allocation per level is
+// slow).  false: no device memory for it -- the level is then left in discovery order (the order is an optimisation).
+static bool ensure_cluster_buf(tlag_engine* e, void** buf, uint64_t* cap, uint64_t bytes, bool slack) {
+  if (bytes <= *cap) return true;
+  dfree(e, *buf); *buf = nullptr; *cap = 0;
+  uint64_t want = slack ? bytes * 2 : bytes;
+  if (dmalloc(e, buf, want) != cudaSuccess) {
+    cudaGetLastError();
+    want = bytes;
+    if (dmalloc(e, buf, want) != cudaSuccess) { cudaGetLastError(); return false; }
+  }
+  *cap = want;
+  return true;
+}
+
 static int cluster_slice(tlag_engine* e, uint64_t first, uint64_t count) {
   static const bool off = getenv("TLAG_NO_SORT") != nullptr;
   if (off || count < 8192 || count > 0xFFFFFFFFull || (e->m.flags & TLAG_F_EXACT)) return TLAG_OK;   // exact: FIFO order is the point
   const uint64_t W = e->m.words_per_state;
-  size_t cub_bytes = 0;
-  cub::DeviceRadixSort::SortPairs(nullptr, cub_bytes, (unsigned long long*)nullptr, (unsigned long long*)nullptr,
-                                  (uint32_t*)nullptr, (uint32_t*)nullptr, (int)0);
-  cub::DeviceRadixSort::SortPairs(nullptr, cub_bytes, (unsigned long long*)nullptr, (unsigned long long*)nullptr,
-                                  (uint32_t*)nullptr, (uint32_t*)nullptr, (unsigned long long)count);
-  // one scratch allocation: keys in/out, idx in/out, cub temp, gathered slice
-  const uint64_t bytes = count * 8 * 2 + count * 4 * 2 + cub_bytes + 256 + count * (W + 2) * 4;
-  if (bytes > e->sort_bytes) {
-    dfree(e, e->d_sort); e->d_sort = nullptr; e->sort_bytes = 0;
-    uint64_t want = bytes * 2;                                  // geometric: levels grow, a re-allocation per level is slow
-    if (dmalloc(e, &e->d_sort, want) != cudaSuccess) {
-      cudaGetLastError();
-      want = bytes;
-      if (dmalloc(e, &e->d_sort, want) != cudaSuccess) { cudaGetLastError(); return TLAG_OK; }   // no memory: skip (optimisation only)
-    }
-    e->sort_bytes = want;
+  const uint64_t cpad = (count + 63) & ~63ull;
+  size_t sort_tmp = 0, list_tmp = 0;
+  {
+    cub::DoubleBuffer<uint32_t> k32(nullptr, nullptr), v32(nullptr, nullptr);
+    cub::DoubleBuffer<unsigned long long> k64(nullptr, nullptr);
+    cub::DeviceRadixSort::SortPairs(nullptr, sort_tmp, k32, v32, (unsigned long long)count);
+    cub::DeviceRadixSort::SortKeys(nullptr, list_tmp, k64, (unsigned long long)count);   // the distinct keys: <= count
   }
+  const size_t cub_bytes = sort_tmp > list_tmp ? sort_tmp : list_tmp;
+  // one scratch allocation: keys | A = (rank, idx) | B = (rank, idx) | records | cub temp.  The distinct keys are listed
+  // and sorted in A and B (as 64-bit words) before the states' ranks are written there.
+  const uint64_t rec_bytes = ((count * (W + 2) * 4) + 255) & ~255ull;
+  if (!ensure_cluster_buf(e, &e->d_sort, &e->sort_bytes, cpad * 8 * 3 + rec_bytes + cub_bytes, true)) return TLAG_OK;
   uint8_t* b = (uint8_t*)e->d_sort;
-  unsigned long long* k_in = (unsigned long long*)b; b += count * 8;
-  unsigned long long* k_out = (unsigned long long*)b; b += count * 8;
-  uint32_t* i_in = (uint32_t*)b; b += count * 4;
-  uint32_t* i_out = (uint32_t*)b; b += count * 4;
-  uint32_t* g_states = (uint32_t*)b; b += count * W * 4;
-  uint32_t* g_parent = (uint32_t*)b; b += count * 4;
-  uint32_t* g_meta = (uint32_t*)b; b += count * 4;
-  b = (uint8_t*)(((uintptr_t)b + 255) & ~(uintptr_t)255);
+  unsigned long long* keys = (unsigned long long*)b; b += cpad * 8;
+  uint8_t* A = b; b += cpad * 8;
+  uint8_t* B = b; b += cpad * 8;
+  uint32_t* rec = (uint32_t*)b; b += rec_bytes;
   void* cub_tmp = b;
   uint32_t* st = e->d_states + first * W;
   const unsigned blocks = (unsigned)((count + 255) / 256);
-  k_sort_keys<<<blocks, 256, 0, e->stream>>>(st, count, (int)W, k_in, i_in);
+  k_cluster_pack<<<blocks, 256, 0, e->stream>>>(st, e->d_parent + first, e->d_meta + first, count, (int)W, rec, keys);
   CK(cudaGetLastError());
-  if (cub::DeviceRadixSort::SortPairs(cub_tmp, cub_bytes, k_in, k_out, i_in, i_out, (unsigned long long)count, 0, 64,
-                                      e->stream) != cudaSuccess) { e->err = "cub sort failed"; return TLAG_ECUDA; }
-  k_gather_slice<<<blocks, 256, 0, e->stream>>>(st, e->d_parent + first, e->d_meta + first, i_out, count, (int)W,
-                                                g_states, g_parent, g_meta);
+  e->launches++;
+
+  // the level's distinct keys; a set past half full is grown 4x and filled again
+  unsigned log2 = e->rset_log2;
+  RankSetCtl hc;
+  unsigned long long *table = nullptr;
+  uint32_t* rank = nullptr;
+  for (;;) {
+    const uint64_t slots = 1ull << log2;
+    if (!ensure_cluster_buf(e, &e->d_rset, &e->rset_bytes, 256 + slots * 12, false)) return TLAG_OK;
+    RankSetCtl* ctl = (RankSetCtl*)e->d_rset;
+    table = (unsigned long long*)((uint8_t*)e->d_rset + 256);
+    rank = (uint32_t*)(table + slots);
+    CK(cudaMemsetAsync(ctl, 0, sizeof(RankSetCtl), e->stream));
+    CK(cudaMemsetAsync(table, 0xFF, slots * 8, e->stream));
+    k_rset_insert<<<blocks, 256, 0, e->stream>>>(keys, count, table, slots - 1, ctl);
+    CK(cudaGetLastError());
+    e->launches++;
+    CK(cudaMemcpyAsync(&hc, ctl, sizeof(hc), cudaMemcpyDeviceToHost, e->stream));
+    CK(cudaStreamSynchronize(e->stream));
+    if (!hc.full) break;
+    log2 += 2;
+  }
+  if (!e->rset_fixed) e->rset_log2 = log2;
+  const uint64_t distinct = (uint64_t)hc.n + hc.has_max;
+  if (distinct <= 1) return TLAG_OK;                  // one key: the stable order is discovery order, already in place
+  const uint64_t slots = 1ull << log2;
+  RankSetCtl* ctl = (RankSetCtl*)e->d_rset;
+
+  // rank of each distinct key = its position in sorted order (a key equal to the empty marker is the largest: rank n)
+  k_rset_list<<<(unsigned)((slots + 255) / 256), 256, 0, e->stream>>>(table, slots, (unsigned long long*)A, ctl);
   CK(cudaGetLastError());
-  CK(cudaMemcpyAsync(st, g_states, count * W * 4, cudaMemcpyDeviceToDevice, e->stream));
-  CK(cudaMemcpyAsync(e->d_parent + first, g_parent, count * 4, cudaMemcpyDeviceToDevice, e->stream));
-  CK(cudaMemcpyAsync(e->d_meta + first, g_meta, count * 4, cudaMemcpyDeviceToDevice, e->stream));
-  e->launches += 3;
+  cub::DoubleBuffer<unsigned long long> dk((unsigned long long*)A, (unsigned long long*)B);
+  size_t tb = cub_bytes;
+  if (cub::DeviceRadixSort::SortKeys(cub_tmp, tb, dk, (unsigned long long)hc.n, 0, 64, e->stream) != cudaSuccess) {
+    e->err = "cub sort failed"; return TLAG_ECUDA;
+  }
+  k_rset_rank<<<(hc.n + 255) / 256, 256, 0, e->stream>>>(dk.Current(), hc.n, table, slots - 1, rank);
+  CK(cudaGetLastError());
+
+  // stable sort of (rank, discovery index) over the rank's bits, then one gather back into the store
+  uint32_t* rank_a = (uint32_t*)A; uint32_t* idx_a = rank_a + cpad;
+  uint32_t* rank_b = (uint32_t*)B; uint32_t* idx_b = rank_b + cpad;
+  k_rank_states<<<blocks, 256, 0, e->stream>>>(keys, count, table, slots - 1, rank, hc.n, rank_a, idx_a);
+  CK(cudaGetLastError());
+  const int end_bit = 32 - __builtin_clz((unsigned)(distinct - 1));
+  cub::DoubleBuffer<uint32_t> rk(rank_a, rank_b), ix(idx_a, idx_b);
+  tb = cub_bytes;
+  if (cub::DeviceRadixSort::SortPairs(cub_tmp, tb, rk, ix, (unsigned long long)count, 0, end_bit, e->stream) != cudaSuccess) {
+    e->err = "cub sort failed"; return TLAG_ECUDA;
+  }
+  k_cluster_gather<<<blocks, 256, 0, e->stream>>>(rec, ix.Current(), count, (int)W, st, e->d_parent + first,
+                                                  e->d_meta + first);
+  CK(cudaGetLastError());
+  e->launches += 4;
+  return TLAG_OK;
+}
+
+// cluster_slice between two events on the engine's stream; the device time goes to out->cluster_ms
+static int timed_cluster_slice(tlag_engine* e, uint64_t first, uint64_t count, tlag_wave_stats* out) {
+  CK(cudaEventRecord(e->ev0, e->stream));
+  int r = cluster_slice(e, first, count);
+  if (r) return r;
+  CK(cudaEventRecord(e->ev1, e->stream));
+  CK(cudaEventSynchronize(e->ev1));
+  float ms = 0;
+  CK(cudaEventElapsedTime(&ms, e->ev0, e->ev1));
+  if (out) out->cluster_ms = ms;
   return TLAG_OK;
 }
 
@@ -845,6 +1040,17 @@ extern "C" int tlag_create(const tlag_model* m, tlag_engine** out) {
     const char* s_ = getenv("TLAG_SL_STAGE");
     e->p.stage = (s_ && *s_) ? (atoi(s_) > 0 ? atoi(s_) : 0) : INT_MAX;
   }
+  // TLAG_RSET_SLOTS=n starts the clustering pass's rank set at n slots (rounded up to a power of two) on every level,
+  // so that a test can make it fill up and grow.  Not a tuning knob.
+  {
+    const char* s_ = getenv("TLAG_RSET_SLOTS");
+    if (s_ && *s_) {
+      const long n = atol(s_);
+      e->rset_log2 = 1;
+      while (e->rset_log2 < 40 && (1L << e->rset_log2) < n) ++e->rset_log2;
+      e->rset_fixed = true;
+    }
+  }
   unsigned log2 = m->table_slots_log2 ? m->table_slots_log2 : 22;
   r = alloc_table(e, log2);
   if (r) return r;
@@ -857,7 +1063,7 @@ extern "C" void tlag_destroy(tlag_engine* e) {
   cudaFree(e->d_code); cudaFree(e->d_cpool); cudaFree(e->d_layout); cudaFree(e->d_ctr); cudaFree(e->d_dig);
   if (e->stream) {
     dfree(e, e->d_states); dfree(e, e->d_parent); dfree(e, e->d_meta); dfree(e, e->d_table);
-    dfree(e, e->d_scratch); dfree(e, e->d_flags); dfree(e, e->d_sort); dfree(e, e->d_sent); dfree(e, e->d_succ);
+    dfree(e, e->d_scratch); dfree(e, e->d_flags); dfree(e, e->d_sort); dfree(e, e->d_rset); dfree(e, e->d_sent); dfree(e, e->d_succ);
     cudaStreamSynchronize(e->stream);
   }
   if (e->p2p_slot >= 0) {                              // exchange buffers and peer mappings are parked, not released
@@ -1121,7 +1327,7 @@ extern "C" int tlag_step(tlag_engine* e, tlag_wave_stats* out) {
   }
   if (n_states > hi) e->depth = e->level + 1;
   if (n_states > hi && e->verdict == TLAG_V_RUNNING) {
-    int rs = cluster_slice(e, hi, n_states - hi);
+    int rs = timed_cluster_slice(e, hi, n_states - hi, out);
     if (rs) return rs;
   }
   {  // head-room for the next level: twice the observed discovered/expanded ratio, at least 4x
@@ -1508,7 +1714,7 @@ extern "C" int tlag_advance_level(tlag_engine* e, tlag_wave_stats* out) {
   if (out) { memset(out, 0, sizeof(*out)); out->level = e->level; out->discovered = n_states - e->hi; out->distinct_total = n_states; out->generated_total = e->generated; out->verdict = e->verdict; }
   if (n_states > e->hi) {
     e->depth = e->level + 1;
-    int rs = cluster_slice(e, e->hi, n_states - e->hi);
+    int rs = timed_cluster_slice(e, e->hi, n_states - e->hi, out);
     if (rs) return rs;
   }
   e->lo = e->hi; e->hi = n_states; e->level += 1;

@@ -1,7 +1,9 @@
 """Where a BFS job's time goes, level by level, on the sliced native kernels: one fixture (tests/golden/*.tlagz) run
 with tlag_step, after `--warmup` untimed runs of the same job on the same engine.  Prints ONE JSON line: per level the
-states expanded, successors generated, states discovered and the wave kernels' time (CUDA events around the level's
-invariant, Next and deadlock kernels), the job's wall time, whether the counts and the digest match the oracle's record,
+states expanded, successors generated, states discovered, the wave kernels' time (CUDA events around the level's
+invariant, Next and deadlock kernels) and the time of the frontier clustering pass that reorders the level's new states
+(`cluster_ms`, with the bytes a reorder cannot avoid -- every record of W words + parent + meta read once and written
+once -- and the rate that gives), the job's wall time, whether the counts and the digest match the oracle's record,
 the TLAG_SL_* switches in effect, and the GPU's name, power limit and maximum SM clock.
 
     python tools/wave_profile.py [MCPaxos3_b4] [--warmup 1] [--max-levels L]
@@ -71,8 +73,11 @@ def main():
             ws = e.step()
             lv += 1
             if ws["expanded"]:
+                reorder = 2 * (cm.W + 2) * 4 * ws["discovered"] if ws["cluster_ms"] > 0 else 0
                 levels.append({k: ws[k] for k in ("level", "expanded", "generated", "discovered")}
-                              | {"kernel_ms": round(ws["kernel_ms"], 3)})
+                              | {"kernel_ms": round(ws["kernel_ms"], 3), "cluster_ms": round(ws["cluster_ms"], 3),
+                                 "reorder_bytes": reorder,
+                                 "reorder_gb_s": round(reorder / ws["cluster_ms"] * 1e-6, 1) if reorder else 0.0})
             if ws["verdict"] != V_RUNNING:
                 break
         return levels if record else None
@@ -88,9 +93,13 @@ def main():
     digest_ok = tuple(e.digest()) == (o2["fp_xor"], o2["fp_sum"])
     e.close()
     kern = sum(lv["kernel_ms"] for lv in levels)
+    clus = sum(lv["cluster_ms"] for lv in levels)
+    reorder = sum(lv["reorder_bytes"] for lv in levels)
     print(json.dumps({"fixture": args.fixture, "W": cm.W, "distinct": r["distinct"], "generated": r["generated"],
                       "depth": r["depth"], "wall_s": round(wall, 4), "kernel_s": round(kern * 1e-3, 4),
-                      "other_s": round(wall - kern * 1e-3, 4), "counts_match_oracle": counts_ok,
+                      "cluster_s": round(clus * 1e-3, 4), "reorder_gb": round(reorder * 1e-9, 2),
+                      "reorder_gb_s": round(reorder / clus * 1e-6, 1) if clus else 0.0,
+                      "other_s": round(wall - (kern + clus) * 1e-3, 4), "counts_match_oracle": counts_ok,
                       "digest_matches_oracle": digest_ok,
                       "switches": switches(),
                       "gpu": gpu_info(os.environ.get("CUDA_VISIBLE_DEVICES", "0").split(",")[0] or "0"),
