@@ -71,6 +71,7 @@ typedef struct {
   float    kernel_ms;            /* device time of the wave kernel (CUDA events)               */
   int32_t  verdict;              /* TLAG_V_RUNNING while the search continues                  */
   float    cluster_ms;           /* device time of the level's frontier clustering pass (events) */
+  uint32_t retries;              /* times the level was rolled back and run again (store or seen-set out of room) */
 } tlag_wave_stats;
 
 typedef struct {

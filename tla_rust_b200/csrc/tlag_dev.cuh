@@ -213,7 +213,7 @@ static __device__ __noinline__ void sl_emit_frame(tlag_sl_cx* cx, const int32_t*
 // warp's buffer; the whole warp later fingerprints and probes the staged successors together (sl_flush, tlag_dev2.cuh),
 // instead of every group of lanes that reaches a site waiting on its own seen-set round trip inside divergent code.
 // Budget: 3.5 KB a warp, 28 KB a 256-thread CTA, so that 4 CTAs per SM take 112 KB of the 228 KB of shared memory.
-// A slot holds the W packed words, the parent index and the meta word; at fewer than 32 slots (W > 25) nothing is staged.
+// A slot holds the W packed words, the parent index and the meta word; at fewer than 32 slots (W > 26) nothing is staged.
 #define TLAG_SL_STAGE_BYTES 3584
 #define TLAG_SL_STAGE_SLOTS ((TLAG_SL_STAGE_BYTES / (4 * (TLAG_SL_W + 2)) / 32) * 32)
 #if TLAG_SL_SCALAR && TLAG_SL_STAGE_SLOTS >= 32

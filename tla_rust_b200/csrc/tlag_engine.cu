@@ -73,6 +73,7 @@ struct tlag_engine {
   int frame_class = 0;
   bool uses_ext = false;            // the image contains LEXLT / SFIND / SINS / EMITD (full interpreter needed)
   bool restarting = false;
+  bool tight = false;               // TLAG_TIGHT_HEADROOM (test hook): store and table sized for no growth, see tlag_create
   double growth_hint = 4.0;
   void* d_sort = nullptr; uint64_t sort_bytes = 0;
   // clustering pass: the rank set ([RankSetCtl | 2^log2 keys | 2^log2 ranks]), its size carried from level to level
@@ -743,9 +744,9 @@ static int alloc_table(tlag_engine* e, unsigned log2) {
 
 static int grow_table_if_needed(tlag_engine* e, uint64_t expected_states) {
   const uint64_t slots = 1ULL << e->table_log2;
-  if (expected_states * 2 <= slots) return TLAG_OK;
+  if (expected_states * (e->tight ? 1 : 2) <= slots) return TLAG_OK;
   unsigned log2 = e->table_log2;
-  while ((1ULL << log2) < expected_states * 4) ++log2;
+  while ((1ULL << log2) < expected_states * (e->tight ? 1 : 4)) ++log2;
   Counters hc;
   CK(cudaMemcpyAsync(&hc, e->d_ctr, sizeof(hc), cudaMemcpyDeviceToHost, e->stream));
   CK(cudaStreamSynchronize(e->stream));
@@ -763,6 +764,7 @@ static int grow_table_if_needed(tlag_engine* e, uint64_t expected_states) {
 static int grow_store_if_needed(tlag_engine* e, uint64_t need) {
   if (need <= e->cap_states) return TLAG_OK;
   uint64_t ncap = e->cap_states;
+  if (e->tight) ncap = need;
   while (ncap < need) ncap *= (ncap < (1ULL << 25) ? 4 : 2);   // few re-allocations while the store is small
   if (e->m.max_states && ncap > e->m.max_states) ncap = e->m.max_states;
   // parent links are 32-bit indices into this rank's store and 0xFFFFFFFF marks an initial state: a store never holds
@@ -999,11 +1001,20 @@ extern "C" int tlag_create(const tlag_model* m, tlag_engine** out) {
   CK(cudaMalloc(&e->d_ctr, sizeof(Counters)));
   int r = reset_counters(e);
   if (r) return r;
+  // TLAG_TIGHT_HEADROOM=1 starts the store at 1024 rows and sizes the store and the seen-set before each level for as many
+  // new states as the level expands, with no slack, and a rerun for exactly what the failed attempt counted: every level
+  // that grows then overflows the store (or, with a small table_slots_log2, fills the table) and is rolled back and
+  // redone (rollback_wave).  Tests use it to run that path; not a tuning knob.
+  {
+    const char* s_ = getenv("TLAG_TIGHT_HEADROOM");
+    e->tight = s_ && *s_ && atoi(s_) != 0;
+  }
   // state store
   uint64_t cap = m->max_states ? m->max_states : (1ULL << 20);
   if (cap < 1024) cap = 1024;
   if (!m->max_states) cap = 1ULL << 20;
   else if (cap > (1ULL << 22)) cap = 1ULL << 22;   // start modest, grow on demand up to max_states
+  if (e->tight) cap = 1024;
   e->cap_states = cap;
   CK(dmalloc(e, &e->d_states, cap * (uint64_t)m->words_per_state * 4));
   CK(dmalloc(e, &e->d_parent, cap * 4));
@@ -1240,15 +1251,15 @@ static void collect_violations(tlag_engine* e, const Counters& hc) {
 }
 
 // Undo a wave that ran out of store or table space: the states it appended are dropped (n_states back to `hi`), the
-// seen-set is rebuilt from the store (it holds fingerprints of the dropped states), counters and violation slots are
-// cleared -- the level is then expanded again from scratch with more room.
+// seen-set is rebuilt from the store (it holds fingerprints of the dropped states), counters, violation slots and the
+// exact replay's stop flag are cleared -- the level is then expanded again from scratch with more room.
 static int rollback_wave(tlag_engine* e, uint64_t hi, uint64_t want_states) {
   Counters hc;
   CK(cudaMemcpy(&hc, e->d_ctr, sizeof(hc), cudaMemcpyDeviceToHost));
-  hc.n_states = hi; hc.generated = 0; hc.work = 0; hc.store_overflow = 0; hc.table_full = 0;
+  hc.n_states = hi; hc.generated = 0; hc.work = 0; hc.store_overflow = 0; hc.table_full = 0; hc.stop = 0;
   hc.viol_inv = hc.viol_assert = hc.viol_trap = hc.viol_deadlock = ~0ULL;
   CK(cudaMemcpy(e->d_ctr, &hc, sizeof(hc), cudaMemcpyHostToDevice));
-  int r = grow_store_if_needed(e, want_states + 4096);
+  int r = grow_store_if_needed(e, e->tight ? want_states : want_states + 4096);
   if (r) return r;
   unsigned log2 = e->table_log2;
   while ((1ULL << log2) < want_states * 2 && log2 < 40) ++log2;
@@ -1275,13 +1286,15 @@ extern "C" int tlag_step(tlag_engine* e, tlag_wave_stats* out) {
     if (out) out->verdict = e->verdict;
     return TLAG_OK;
   }
-  int r = grow_store_if_needed(e, hi + (uint64_t)((double)(hi - lo) * e->growth_hint) + 4096);
+  int r = grow_store_if_needed(e, e->tight ? hi + (hi - lo) : hi + (uint64_t)((double)(hi - lo) * e->growth_hint) + 4096);
   if (r) return r;
-  r = grow_table_if_needed(e, hi + (uint64_t)((double)(hi - lo) * (e->growth_hint > 4.0 ? e->growth_hint * 0.5 : 2.0)));
+  r = grow_table_if_needed(e, e->tight ? hi + (hi - lo)
+                                       : hi + (uint64_t)((double)(hi - lo) * (e->growth_hint > 4.0 ? e->growth_hint * 0.5 : 2.0)));
   if (r) return r;
   Counters hc;
   float ms = 0;
-  for (int attempt = 0;; ++attempt) {
+  int attempt = 0;
+  for (;; ++attempt) {
     CK(cudaMemsetAsync(&e->d_ctr->work, 0, 8, e->stream));
     CK(cudaEventRecord(e->ev0, e->stream));
     cudaError_t ce = launch_wave<0>(e, lo, hi);
@@ -1296,7 +1309,7 @@ extern "C" int tlag_step(tlag_engine* e, tlag_wave_stats* out) {
     // The head-room heuristics were too tight for this level (its discovered / expanded ratio jumped): n_states kept
     // counting past the capacity, so it says how much room the level needs.  Redo the level with that much, twice over.
     const uint64_t need = hc.n_states > hi ? hc.n_states : hi;
-    const uint64_t want = hi + (need - hi) * 2 + 4096;
+    const uint64_t want = e->tight ? need : hi + (need - hi) * 2 + 4096;
     if (attempt >= 3 || (e->m.max_states && need > e->m.max_states) || need > 0xFFFFFFFEull) {
       e->err = hc.store_overflow ? "state store overflow: raise max_states (or the model needs more than 2^32 - 2 states per GPU)"
                                  : "seen-set table full";
@@ -1304,7 +1317,7 @@ extern "C" int tlag_step(tlag_engine* e, tlag_wave_stats* out) {
     }
     r = rollback_wave(e, hi, want);
     if (r) return r;
-    if (e->cap_states < need + 1024) { e->err = "state store overflow: not enough device memory for this level"; return TLAG_ENOMEM; }
+    if (e->cap_states < need + (e->tight ? 0 : 1024)) { e->err = "state store overflow: not enough device memory for this level"; return TLAG_ENOMEM; }
   }
   e->dev_seconds += ms * 1e-3;
   const uint64_t gen_wave = hc.generated;
@@ -1324,6 +1337,7 @@ extern "C" int tlag_step(tlag_engine* e, tlag_wave_stats* out) {
     out->level = e->level; out->expanded = hi - lo; out->generated = gen_wave;
     out->discovered = n_states - hi; out->distinct_total = n_states; out->generated_total = e->generated;
     out->kernel_ms = ms;
+    out->retries = (uint32_t)attempt;
   }
   if (n_states > hi) e->depth = e->level + 1;
   if (n_states > hi && e->verdict == TLAG_V_RUNNING) {

@@ -44,7 +44,8 @@ class TlagModel(C.Structure):
 class WaveStats(C.Structure):
     _fields_ = [("level", C.c_uint64), ("expanded", C.c_uint64), ("generated", C.c_uint64),
                 ("discovered", C.c_uint64), ("distinct_total", C.c_uint64), ("generated_total", C.c_uint64),
-                ("kernel_ms", C.c_float), ("verdict", C.c_int32), ("cluster_ms", C.c_float)]
+                ("kernel_ms", C.c_float), ("verdict", C.c_int32), ("cluster_ms", C.c_float),
+                ("retries", C.c_uint32)]
 
     def as_dict(self):
         return {f: getattr(self, f) for f, _ in self._fields_}
