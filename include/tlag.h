@@ -156,6 +156,65 @@ int  tlag_p2p_level(tlag_engine *e, uint64_t n_chunks, uint64_t chunk_states, ui
  * with smaller chunks. */
 int  tlag_p2p_rollback(tlag_engine *e);
 
+/* ---- liveness building blocks: strongly connected components and fair cycles of a state graph ---------------------
+ * Standalone calls (no engine): the caller passes the graph as a host edge list over states 0..n_states-1; each call
+ * copies it to the device, works there and returns.  Self-loops are ignored (a self-loop cannot satisfy <<A>>_v; the
+ * implicit stuttering step of every state stands for it), so every SCC, a single state included, carries a cycle.
+ * An edge endpoint >= n_states is TLAG_EINVAL.  The calling thread's current CUDA device is the same on return.
+ * Errors: negative return codes + tlag_graph_last_error (per host thread). */
+typedef struct {
+  uint64_t n_states;             /* < 2^32 - 1                                                  */
+  uint64_t n_edges;              /* < 2^32                                                      */
+  const uint32_t *src, *dst;     /* n_edges state indices each                                  */
+  const uint32_t *edge_label;    /* n_edges words: bit b = the edge satisfies <<A_b>>_v (NULL = all 0) */
+  const uint32_t *state_label;   /* n_states words: state predicates, ENABLED bits (NULL = all 0) */
+  const uint8_t  *state_mask;    /* nonzero = the state is in the restricted graph (NULL = all) */
+  const uint8_t  *edge_mask;     /* nonzero = the edge is in the restricted graph (NULL = all)  */
+  int32_t device;                /* CUDA device ordinal                                         */
+} tlag_graph;
+
+/* SCC decomposition of the restricted graph: scc_out[v] = id of v's component (the index of one of its states), or
+ * 0xFFFFFFFF for a state outside the mask.  Trim, then forward-backward from the state of largest degree product,
+ * then colour propagation for the rest.  device_ms: device time of the edge compaction, the CSR build and the
+ * decomposition (CUDA events; the host<->device copies are not counted). */
+int  tlag_scc(const tlag_graph *g, uint32_t *scc_out, uint64_t *n_scc_out, float *device_ms);
+
+enum { TLAG_FAIR_WF = 0, TLAG_FAIR_SF = 1 };
+typedef struct {
+  uint32_t kind;                 /* TLAG_FAIR_WF / TLAG_FAIR_SF                                 */
+  uint32_t enabled_bit;          /* state-label bit of ENABLED <<A>>_v                          */
+  uint32_t action_bit;           /* edge-label bit of <<A>>_v                                   */
+  uint32_t reserved;
+} tlag_fairness;
+
+typedef struct {
+  const tlag_fairness *fair;     /* fairness conditions every accepted cycle must satisfy       */
+  uint32_t n_fair;
+  uint32_t need_clear;           /* state-label bits: an accepted SCC holds, for each bit, a state where it is clear
+                                  * (the ~Y state of every <>[]Y disjunct of the obligation)    */
+  const uint8_t *seeds;          /* NULL: every accepted SCC counts; else only those reachable in the restricted
+                                  * graph from a state with seeds[v] != 0 (P ~> Q: P /\ ~Q states; <>P: initial ~P) */
+} tlag_fair_query;
+
+typedef struct {
+  int32_t  violated;             /* 1 = a (reachable) accepted SCC exists: the obligation fails */
+  uint32_t witness;              /* smallest state of such an SCC (0xFFFFFFFF if none)          */
+  uint64_t fair_sccs;            /* accepted SCCs, reachable or not                             */
+  uint32_t rounds;               /* SCC decompositions run (Emerson-Lei refinements + 1)        */
+  float    device_ms;            /* device time from the edge compaction on (CUDA events, copies excluded) */
+} tlag_fair_result;
+
+/* Fair-cycle search (Emerson-Lei) on the restricted graph.  An SCC C is accepted when, for every condition,
+ *   WF: some state of C has ~EN, or some edge inside C has the action bit;
+ *   SF: no state of C has EN, or some edge inside C has the action bit;
+ * and C holds a state with each need_clear bit clear.  C failing a WF or need_clear test is dropped; C failing only
+ * SF tests loses its EN states and the rest is decomposed again, to a fixpoint.  scc_out[v] = accepted SCC id of v,
+ * else 0xFFFFFFFF (NULL: not returned).  The cycle through every state and edge of an accepted SCC is fair and
+ * violates the obligation the masks and need_clear encode.  Provisional: it uploads the graph and builds both CSRs on
+ * every call; the obligation check on a graph the engine builds in device memory will replace it. */
+int  tlag_fair_cycles(const tlag_graph *g, const tlag_fair_query *q, uint32_t *scc_out, tlag_fair_result *out);
+const char *tlag_graph_last_error(void);
+
 #ifdef __cplusplus
 }
 #endif

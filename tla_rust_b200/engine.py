@@ -380,6 +380,101 @@ class Engine:
         return ws.as_dict()
 
 
+# ---- liveness building blocks on a caller-provided state graph (include/tlag.h: tlag_scc, tlag_fair_cycles)
+NO_SCC = 0xFFFFFFFF             # scc id of a state outside the mask / outside every accepted SCC
+FAIR_KINDS = {"WF": 0, "SF": 1}
+
+
+class TlagGraph(C.Structure):
+    _fields_ = [("n_states", C.c_uint64), ("n_edges", C.c_uint64), ("src", C.c_void_p), ("dst", C.c_void_p),
+                ("edge_label", C.c_void_p), ("state_label", C.c_void_p), ("state_mask", C.c_void_p),
+                ("edge_mask", C.c_void_p), ("device", C.c_int32)]
+
+
+class TlagFairness(C.Structure):
+    _fields_ = [("kind", C.c_uint32), ("enabled_bit", C.c_uint32), ("action_bit", C.c_uint32), ("reserved", C.c_uint32)]
+
+
+class TlagFairQuery(C.Structure):
+    _fields_ = [("fair", C.c_void_p), ("n_fair", C.c_uint32), ("need_clear", C.c_uint32), ("seeds", C.c_void_p)]
+
+
+class TlagFairResult(C.Structure):
+    _fields_ = [("violated", C.c_int32), ("witness", C.c_uint32), ("fair_sccs", C.c_uint64), ("rounds", C.c_uint32),
+                ("device_ms", C.c_float)]
+
+
+def _graph_lib():
+    L = load_library()
+    if not hasattr(L, "_graph_bound"):
+        L.tlag_graph_last_error.restype = C.c_char_p
+        L._graph_bound = True
+    return L
+
+
+def _graph_call(L, rc, what):
+    if rc != 0:
+        raise EngineError(f"{what}: rc={rc}: {L.tlag_graph_last_error().decode()}")
+
+
+def _graph_struct(n_states, src, dst, edge_label, state_label, state_mask, edge_mask, device):
+    """-> (tlag_graph, arrays it points into: keep them alive for the call)"""
+    src = np.ascontiguousarray(src, dtype=np.uint32)
+    dst = np.ascontiguousarray(dst, dtype=np.uint32)
+    if src.shape != dst.shape or src.ndim != 1:
+        raise ValueError("src and dst must be 1-D arrays of one length")
+    if src.size and max(int(src.max()), int(dst.max())) >= n_states:
+        raise ValueError("edge endpoint >= n_states")
+    keep = [src, dst]
+
+    def arr(a, dtype, size, what):
+        if a is None:
+            return None
+        a = np.ascontiguousarray(a, dtype=dtype)
+        if a.shape != (size,):
+            raise ValueError(f"{what} must have shape ({size},)")
+        keep.append(a)
+        return a.ctypes.data
+
+    g = TlagGraph(n_states, src.size, src.ctypes.data, dst.ctypes.data,
+                  arr(edge_label, np.uint32, src.size, "edge_label"), arr(state_label, np.uint32, n_states, "state_label"),
+                  arr(state_mask, np.uint8, n_states, "state_mask"), arr(edge_mask, np.uint8, src.size, "edge_mask"), device)
+    return g, keep
+
+
+def scc(n_states, src, dst, state_mask=None, edge_mask=None, device=0):
+    """SCC decomposition on the GPU of the graph restricted to the masks (self-loops ignored).
+    -> (component id per state, NO_SCC outside the mask; number of components; device ms)"""
+    L = _graph_lib()
+    g, keep = _graph_struct(n_states, src, dst, None, None, state_mask, edge_mask, device)
+    out = np.empty(n_states, dtype=np.uint32)
+    n, ms = C.c_uint64(), C.c_float()
+    _graph_call(L, L.tlag_scc(C.byref(g), out.ctypes.data_as(C.c_void_p), C.byref(n), C.byref(ms)), "tlag_scc")
+    return out, int(n.value), float(ms.value)
+
+
+def fair_cycles(n_states, src, dst, edge_label=None, state_label=None, state_mask=None, edge_mask=None, fairness=(),
+                need_clear=0, seeds=None, device=0):
+    """Fair-cycle search (Emerson-Lei) on the GPU; see tlag_fair_cycles in include/tlag.h.
+    fairness: (kind "WF"/"SF", ENABLED bit of state_label, action bit of edge_label) triples.
+    -> dict(violated, witness, fair_sccs, rounds, device_ms, scc = accepted SCC id per state or NO_SCC)"""
+    L = _graph_lib()
+    g, keep = _graph_struct(n_states, src, dst, edge_label, state_label, state_mask, edge_mask, device)
+    fair = (TlagFairness * max(1, len(fairness)))(*[TlagFairness(FAIR_KINDS[k], en, act, 0) for k, en, act in fairness])
+    sd = None
+    if seeds is not None:
+        sd = np.ascontiguousarray(seeds, dtype=np.uint8)
+        if sd.shape != (n_states,):
+            raise ValueError(f"seeds must have shape ({n_states},)")
+    q = TlagFairQuery(C.addressof(fair), len(fairness), need_clear, None if sd is None else sd.ctypes.data)
+    out = np.empty(n_states, dtype=np.uint32)
+    r = TlagFairResult()
+    _graph_call(L, L.tlag_fair_cycles(C.byref(g), C.byref(q), out.ctypes.data_as(C.c_void_p), C.byref(r)),
+                "tlag_fair_cycles")
+    return {"violated": bool(r.violated), "witness": None if r.witness == NO_SCC else int(r.witness),
+            "fair_sccs": int(r.fair_sccs), "rounds": int(r.rounds), "device_ms": float(r.device_ms), "scc": out}
+
+
 class ProbeOnlyModel:
     """Minimal stand-in CompiledModel for K1-only use (tlag_probe_batch on W-word states)."""
 
