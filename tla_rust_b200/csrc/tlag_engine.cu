@@ -730,6 +730,45 @@ static cudaError_t launch_wave(tlag_engine* e, uint64_t lo, uint64_t hi) {
 
 #endif
 
+// The counter block after everything queued on the engine's stream so far.  The stream is non-blocking, so a copy on
+// the legacy stream would not wait for that work: this is the only copy of d_ctr to the host.
+static cudaError_t read_counters(tlag_engine* e, Counters* hc) {
+  cudaError_t r = cudaMemcpyAsync(hc, e->d_ctr, sizeof(*hc), cudaMemcpyDeviceToHost, e->stream);
+  return r != cudaSuccess ? r : cudaStreamSynchronize(e->stream);
+}
+
+// The counters of a store of n_states states that has discovered nothing since: zero, and the violation slots (minimum
+// keys) at "none"
+static cudaError_t reset_counters(tlag_engine* e, uint64_t n_states) {
+  Counters hc;
+  memset(&hc, 0, sizeof(hc));
+  hc.n_states = n_states;
+  hc.viol_inv = hc.viol_assert = hc.viol_trap = hc.viol_deadlock = ~0ULL;
+  return cudaMemcpyAsync(e->d_ctr, &hc, sizeof(hc), cudaMemcpyHostToDevice, e->stream);   // pageable: staged before return
+}
+
+// enqueue() between two events on the engine's stream; waits for it and returns its device time in *ms.  With hc the
+// counters are read in the same synchronisation.
+template <class F>
+static int timed(tlag_engine* e, float* ms, Counters* hc, F&& enqueue) {
+  CK(cudaEventRecord(e->ev0, e->stream));
+  int r = enqueue();
+  if (r) return r;
+  CK(cudaEventRecord(e->ev1, e->stream));
+  if (hc) CK(read_counters(e, hc));
+  else CK(cudaEventSynchronize(e->ev1));
+  CK(cudaEventElapsedTime(ms, e->ev0, e->ev1));
+  return TLAG_OK;
+}
+
+// A snapshot's store overflow or full seen-set as TLAG_ENOMEM with its message in e->err (store_msg null: the store is
+// not checked)
+static int overflow_error(tlag_engine* e, const Counters& hc, const char* store_msg, const char* table_msg) {
+  if (store_msg && hc.store_overflow) { e->err = store_msg; return TLAG_ENOMEM; }
+  if (hc.table_full) { e->err = table_msg; return TLAG_ENOMEM; }
+  return TLAG_OK;
+}
+
 static int alloc_table(tlag_engine* e, unsigned log2) {
   if (e->d_table) dfree(e, e->d_table);
   e->d_table = nullptr;
@@ -748,8 +787,7 @@ static int grow_table_if_needed(tlag_engine* e, uint64_t expected_states) {
   unsigned log2 = e->table_log2;
   while ((1ULL << log2) < expected_states * (e->tight ? 1 : 4)) ++log2;
   Counters hc;
-  CK(cudaMemcpyAsync(&hc, e->d_ctr, sizeof(hc), cudaMemcpyDeviceToHost, e->stream));
-  CK(cudaStreamSynchronize(e->stream));
+  CK(read_counters(e, &hc));
   int r = alloc_table(e, log2);
   if (r) return r;
   const uint64_t n = hc.n_states;
@@ -787,8 +825,7 @@ static int grow_store_if_needed(tlag_engine* e, uint64_t need) {
   CK(dmalloc(e, &np, ncap * 4));
   CK(dmalloc(e, &nm, ncap * 4));
   Counters hc;
-  CK(cudaMemcpyAsync(&hc, e->d_ctr, sizeof(hc), cudaMemcpyDeviceToHost, e->stream));
-  CK(cudaStreamSynchronize(e->stream));
+  CK(read_counters(e, &hc));
   const uint64_t n = hc.n_states;
   CK(cudaMemcpyAsync(ns, e->d_states, n * (uint64_t)e->m.words_per_state * 4, cudaMemcpyDeviceToDevice, e->stream));
   CK(cudaMemcpyAsync(np, e->d_parent, n * 4, cudaMemcpyDeviceToDevice, e->stream));
@@ -799,6 +836,12 @@ static int grow_store_if_needed(tlag_engine* e, uint64_t need) {
   e->cap_states = ncap;
   e->p.states = ns; e->p.parent = np; e->p.meta = nm; e->p.cap_states = ncap;
   return TLAG_OK;
+}
+
+// room for a level before it runs: the store for store_need states, the seen-set for table_need
+static int reserve_level(tlag_engine* e, uint64_t store_need, uint64_t table_need) {
+  int r = grow_store_if_needed(e, store_need);
+  return r ? r : grow_table_if_needed(e, table_need);
 }
 
 // Grows a clustering buffer to at least `bytes` (geometrically when `slack`: levels grow, a re-allocation per level is
@@ -901,28 +944,6 @@ static int cluster_slice(tlag_engine* e, uint64_t first, uint64_t count) {
   return TLAG_OK;
 }
 
-// cluster_slice between two events on the engine's stream; the device time goes to out->cluster_ms
-static int timed_cluster_slice(tlag_engine* e, uint64_t first, uint64_t count, tlag_wave_stats* out) {
-  CK(cudaEventRecord(e->ev0, e->stream));
-  int r = cluster_slice(e, first, count);
-  if (r) return r;
-  CK(cudaEventRecord(e->ev1, e->stream));
-  CK(cudaEventSynchronize(e->ev1));
-  float ms = 0;
-  CK(cudaEventElapsedTime(&ms, e->ev0, e->ev1));
-  if (out) out->cluster_ms = ms;
-  return TLAG_OK;
-}
-
-// the counters of a search that has discovered nothing: zero, and the violation slots (minimum keys) at "none"
-static int reset_counters(tlag_engine* e) {
-  Counters hc;
-  memset(&hc, 0, sizeof(hc));
-  hc.viol_inv = hc.viol_assert = hc.viol_trap = hc.viol_deadlock = ~0ULL;
-  CK(cudaMemcpyAsync(e->d_ctr, &hc, sizeof(hc), cudaMemcpyHostToDevice, e->stream));   // pageable: staged before return
-  return TLAG_OK;
-}
-
 // Route mode with several ranks: the direct-mapped cache of the fingerprints this rank has routed (2^26 x 8 B = 512 MB).
 // It is only a filter: without memory for it, or with TLAG_NO_SENT_CACHE set, every successor is routed.
 static int ensure_sent_cache(tlag_engine* e) {
@@ -999,8 +1020,7 @@ extern "C" int tlag_create(const tlag_model* m, tlag_engine** out) {
   CK(cudaMalloc(&e->d_layout, (size_t)(m->n_slots ? m->n_slots : 1) * sizeof(tlag_slot)));
   CK(cudaMemcpy(e->d_layout, m->layout, (size_t)m->n_slots * sizeof(tlag_slot), cudaMemcpyHostToDevice));
   CK(cudaMalloc(&e->d_ctr, sizeof(Counters)));
-  int r = reset_counters(e);
-  if (r) return r;
+  CK(reset_counters(e, 0));
   // TLAG_TIGHT_HEADROOM=1 starts the store at 1024 rows and sizes the store and the seen-set before each level for as many
   // new states as the level expands, with no slack, and a rerun for exactly what the failed attempt counted: every level
   // that grows then overflows the store (or, with a small table_slots_log2, fills the table) and is rolled back and
@@ -1063,7 +1083,7 @@ extern "C" int tlag_create(const tlag_model* m, tlag_engine** out) {
     }
   }
   unsigned log2 = m->table_slots_log2 ? m->table_slots_log2 : 22;
-  r = alloc_table(e, log2);
+  int r = alloc_table(e, log2);
   if (r) return r;
   CK(cudaStreamSynchronize(e->stream));
   return TLAG_OK;
@@ -1120,18 +1140,12 @@ static int launch_probe(tlag_engine* e, const uint32_t* d_states, uint64_t n, ui
 
 extern "C" int tlag_probe_batch_device(tlag_engine* e, uint64_t d_states, uint64_t n, uint64_t d_is_new, float* kernel_ms) {
   if (!e) return TLAG_EINVAL;
-  CK(cudaEventRecord(e->ev0, e->stream));
-  int r = launch_probe(e, (const uint32_t*)(uintptr_t)d_states, n, (uint8_t*)(uintptr_t)d_is_new);
-  if (r) return r;
-  CK(cudaEventRecord(e->ev1, e->stream));
-  CK(cudaEventSynchronize(e->ev1));
-  float ms = 0;
-  CK(cudaEventElapsedTime(&ms, e->ev0, e->ev1));
-  if (kernel_ms) *kernel_ms = ms;
   Counters hc;
-  CK(cudaMemcpy(&hc, e->d_ctr, sizeof(hc), cudaMemcpyDeviceToHost));
-  if (hc.table_full) { e->err = "seen-set table is full"; return TLAG_ENOMEM; }
-  return TLAG_OK;
+  float ms = 0;
+  int r = timed(e, &ms, &hc, [&] { return launch_probe(e, (const uint32_t*)(uintptr_t)d_states, n, (uint8_t*)(uintptr_t)d_is_new); });
+  if (r) return r;
+  if (kernel_ms) *kernel_ms = ms;
+  return overflow_error(e, hc, nullptr, "seen-set table is full");
 }
 
 extern "C" int tlag_probe_batch(tlag_engine* e, const uint32_t* states, uint64_t n, uint8_t* is_new) {
@@ -1144,11 +1158,9 @@ extern "C" int tlag_probe_batch(tlag_engine* e, const uint32_t* states, uint64_t
   r = launch_probe(e, e->d_scratch, n, e->d_flags);
   if (r) return r;
   CK(cudaMemcpyAsync(is_new, e->d_flags, n, cudaMemcpyDeviceToHost, e->stream));
-  CK(cudaStreamSynchronize(e->stream));
   Counters hc;
-  CK(cudaMemcpy(&hc, e->d_ctr, sizeof(hc), cudaMemcpyDeviceToHost));
-  if (hc.table_full) { e->err = "seen-set table is full"; return TLAG_ENOMEM; }
-  return TLAG_OK;
+  CK(read_counters(e, &hc));
+  return overflow_error(e, hc, nullptr, "seen-set table is full");
 }
 
 extern "C" int tlag_reset_table(tlag_engine* e) {
@@ -1162,9 +1174,7 @@ extern "C" int tlag_seed(tlag_engine* e, const uint32_t* states, uint64_t n) {
   if (!e || (!states && n)) return TLAG_EINVAL;
   if (e->level != 0) { e->err = "tlag_seed after the search started"; return TLAG_ESTATE; }
   const uint64_t W = e->m.words_per_state;
-  int r = grow_store_if_needed(e, e->hi + n + 1024);
-  if (r) return r;
-  r = grow_table_if_needed(e, e->hi + n);
+  int r = reserve_level(e, e->hi + n + 1024, e->hi + n);
   if (r) return r;
   if (n) {
     // records: W words + parent(-1) + meta(action -1)
@@ -1188,10 +1198,9 @@ extern "C" int tlag_seed(tlag_engine* e, const uint32_t* states, uint64_t n) {
     }
     e->launches++;
     CK(cudaGetLastError());
-    CK(cudaStreamSynchronize(e->stream));
   }
   Counters hc;
-  CK(cudaMemcpy(&hc, e->d_ctr, sizeof(hc), cudaMemcpyDeviceToHost));
+  CK(read_counters(e, &hc));
   e->generated += n;
   e->hi = hc.n_states;
   e->init_states = hc.n_states;
@@ -1202,8 +1211,7 @@ extern "C" int tlag_seed(tlag_engine* e, const uint32_t* states, uint64_t n) {
 // Forget everything discovered and start again from the retained initial states (bench loops).
 extern "C" int tlag_restart(tlag_engine* e) {
   if (!e) return TLAG_EINVAL;
-  int r = reset_counters(e);
-  if (r) return r;
+  CK(reset_counters(e, 0));
   CK(cudaMemsetAsync(e->d_table, 0, (1ULL << e->table_log2) * 8, e->stream));
   if (e->d_sent) CK(cudaMemsetAsync(e->d_sent, 0, (e->p.sent_mask + 1) * 8, e->stream));
   CK(cudaStreamSynchronize(e->stream));
@@ -1212,7 +1220,7 @@ extern "C" int tlag_restart(tlag_engine* e) {
   e->kg_verdict = 0;
   e->restarting = true;
   const uint64_t W = e->m.words_per_state;
-  r = tlag_seed(e, e->h_init.data(), e->h_init.size() / W);
+  int r = tlag_seed(e, e->h_init.data(), e->h_init.size() / W);
   e->restarting = false;
   return r;
 }
@@ -1250,15 +1258,71 @@ static void collect_violations(tlag_engine* e, const Counters& hc) {
   else if (kind == TLAG_V_INVARIANT) e->detail = (int)(hc.viol_inv & 0xFFFFF);
 }
 
+// the first level call of a search: the frontier is the seeded initial states
+static void start_search(tlag_engine* e) {
+  if (e->level == 0) { e->level = 1; e->lo = 0; e->depth = e->hi > 0 ? 1 : 0; }
+}
+
+// the search reached its fixpoint: OK, or under TLAG_F_KEEP_GOING the first violation it went past
+static void settle_verdict(tlag_engine* e) {
+  e->verdict = e->kg_verdict ? e->kg_verdict : TLAG_V_OK;
+  if (e->kg_verdict) { e->detail = e->kg_detail; e->detail2 = e->kg_detail2; e->viol_idx = e->kg_idx; }
+}
+
+// End of a wave, from the counters read after it: its `generated` moves to the host total (and is cleared on the
+// device), a violation becomes the verdict, and out gets the wave's numbers.  keep_going: the first violation is
+// remembered, the device slots are cleared and the search goes on.
+static int account_wave(tlag_engine* e, const Counters& hc, bool keep_going, uint64_t expanded, float ms,
+                        tlag_wave_stats* out) {
+  e->generated += hc.generated;
+  CK(cudaMemsetAsync(&e->d_ctr->generated, 0, 8, e->stream));
+  collect_violations(e, hc);
+  if (keep_going && e->verdict != TLAG_V_RUNNING) {
+    if (!e->kg_verdict) { e->kg_verdict = e->verdict; e->kg_detail = e->detail; e->kg_detail2 = e->detail2; e->kg_idx = e->viol_idx; }
+    e->verdict = TLAG_V_RUNNING;
+    const unsigned long long ones[4] = {~0ULL, ~0ULL, ~0ULL, ~0ULL};
+    CK(cudaMemcpyAsync(&e->d_ctr->viol_inv, ones, sizeof(ones), cudaMemcpyHostToDevice, e->stream));
+    CK(cudaStreamSynchronize(e->stream));
+  }
+  if (out) {
+    out->level = e->level; out->expanded = expanded; out->generated = hc.generated;
+    out->distinct_total = hc.n_states; out->generated_total = e->generated; out->kernel_ms = ms;
+    out->verdict = e->verdict;
+  }
+  return TLAG_OK;
+}
+
+// head-room for the next level: twice the observed discovered/expanded ratio, at least 4x
+static void note_growth(tlag_engine* e, uint64_t expanded, uint64_t discovered) {
+  const double ratio = (double)discovered / (double)(expanded ? expanded : 1);
+  e->growth_hint = ratio * 2.0 > 4.0 ? ratio * 2.0 : 4.0;
+}
+
+// End of a level whose store now holds n_states states: the slice it appended (if any) sets the depth and, with
+// cluster, is put in clustering order (device time in out->cluster_ms); then it becomes the frontier.
+static int close_level(tlag_engine* e, uint64_t n_states, bool cluster, tlag_wave_stats* out) {
+  if (out) {
+    out->level = e->level; out->discovered = n_states - e->hi; out->distinct_total = n_states;
+    out->generated_total = e->generated; out->verdict = e->verdict;
+  }
+  if (n_states > e->hi) {
+    e->depth = e->level + 1;
+    if (cluster) {
+      float ms = 0;
+      int r = timed(e, &ms, nullptr, [&] { return cluster_slice(e, e->hi, n_states - e->hi); });
+      if (r) return r;
+      if (out) out->cluster_ms = ms;
+    }
+  }
+  e->lo = e->hi; e->hi = n_states; e->level += 1;
+  return TLAG_OK;
+}
+
 // Undo a wave that ran out of store or table space: the states it appended are dropped (n_states back to `hi`), the
-// seen-set is rebuilt from the store (it holds fingerprints of the dropped states), counters, violation slots and the
-// exact replay's stop flag are cleared -- the level is then expanded again from scratch with more room.
+// seen-set is rebuilt from the store (it holds fingerprints of the dropped states) and every other counter is reset --
+// the level is then expanded again from scratch with more room.
 static int rollback_wave(tlag_engine* e, uint64_t hi, uint64_t want_states) {
-  Counters hc;
-  CK(cudaMemcpy(&hc, e->d_ctr, sizeof(hc), cudaMemcpyDeviceToHost));
-  hc.n_states = hi; hc.generated = 0; hc.work = 0; hc.store_overflow = 0; hc.table_full = 0; hc.stop = 0;
-  hc.viol_inv = hc.viol_assert = hc.viol_trap = hc.viol_deadlock = ~0ULL;
-  CK(cudaMemcpy(e->d_ctr, &hc, sizeof(hc), cudaMemcpyHostToDevice));
+  CK(reset_counters(e, hi));
   int r = grow_store_if_needed(e, e->tight ? want_states : want_states + 4096);
   if (r) return r;
   unsigned log2 = e->table_log2;
@@ -1277,82 +1341,47 @@ static int rollback_wave(tlag_engine* e, uint64_t hi, uint64_t want_states) {
 extern "C" int tlag_step(tlag_engine* e, tlag_wave_stats* out) {
   if (!e) return TLAG_EINVAL;
   if (out) memset(out, 0, sizeof(*out));
-  if (e->level == 0) { e->level = 1; e->lo = 0; e->depth = e->hi > 0 ? 1 : 0; }
+  start_search(e);
   if (e->verdict != TLAG_V_RUNNING) { if (out) out->verdict = e->verdict; return TLAG_OK; }
   const uint64_t lo = e->lo, hi = e->hi;
   if (lo >= hi) {
-    e->verdict = e->kg_verdict ? e->kg_verdict : TLAG_V_OK;
-    if (e->kg_verdict) { e->detail = e->kg_detail; e->detail2 = e->kg_detail2; e->viol_idx = e->kg_idx; }
+    settle_verdict(e);
     if (out) out->verdict = e->verdict;
     return TLAG_OK;
   }
-  int r = grow_store_if_needed(e, e->tight ? hi + (hi - lo) : hi + (uint64_t)((double)(hi - lo) * e->growth_hint) + 4096);
-  if (r) return r;
-  r = grow_table_if_needed(e, e->tight ? hi + (hi - lo)
-                                       : hi + (uint64_t)((double)(hi - lo) * (e->growth_hint > 4.0 ? e->growth_hint * 0.5 : 2.0)));
+  int r = reserve_level(e, e->tight ? hi + (hi - lo) : hi + (uint64_t)((double)(hi - lo) * e->growth_hint) + 4096,
+                        e->tight ? hi + (hi - lo)
+                                 : hi + (uint64_t)((double)(hi - lo) * (e->growth_hint > 4.0 ? e->growth_hint * 0.5 : 2.0)));
   if (r) return r;
   Counters hc;
   float ms = 0;
   int attempt = 0;
   for (;; ++attempt) {
     CK(cudaMemsetAsync(&e->d_ctr->work, 0, 8, e->stream));
-    CK(cudaEventRecord(e->ev0, e->stream));
-    cudaError_t ce = launch_wave<0>(e, lo, hi);
-    if (ce != cudaSuccess) { e->err = std::string("wave launch: ") + cudaGetErrorString(ce); return TLAG_ECUDA; }
-    CK(cudaEventRecord(e->ev1, e->stream));
-    CK(cudaMemcpyAsync(&hc, e->d_ctr, sizeof(hc), cudaMemcpyDeviceToHost, e->stream));
-    CK(cudaStreamSynchronize(e->stream));
     float ms1 = 0;
-    CK(cudaEventElapsedTime(&ms1, e->ev0, e->ev1));
+    r = timed(e, &ms1, &hc, [&] { CK(launch_wave<0>(e, lo, hi)); return TLAG_OK; });
+    if (r) return r;
     ms += ms1;
     if (!hc.store_overflow && !hc.table_full) break;
     // The head-room heuristics were too tight for this level (its discovered / expanded ratio jumped): n_states kept
     // counting past the capacity, so it says how much room the level needs.  Redo the level with that much, twice over.
     const uint64_t need = hc.n_states > hi ? hc.n_states : hi;
     const uint64_t want = e->tight ? need : hi + (need - hi) * 2 + 4096;
-    if (attempt >= 3 || (e->m.max_states && need > e->m.max_states) || need > 0xFFFFFFFEull) {
-      e->err = hc.store_overflow ? "state store overflow: raise max_states (or the model needs more than 2^32 - 2 states per GPU)"
-                                 : "seen-set table full";
-      return TLAG_ENOMEM;
-    }
+    if (attempt >= 3 || (e->m.max_states && need > e->m.max_states) || need > 0xFFFFFFFEull)
+      return overflow_error(e, hc, "state store overflow: raise max_states (or the model needs more than 2^32 - 2 states per GPU)",
+                            "seen-set table full");
     r = rollback_wave(e, hi, want);
     if (r) return r;
     if (e->cap_states < need + (e->tight ? 0 : 1024)) { e->err = "state store overflow: not enough device memory for this level"; return TLAG_ENOMEM; }
   }
   e->dev_seconds += ms * 1e-3;
-  const uint64_t gen_wave = hc.generated;
-  e->generated += gen_wave;
-  CK(cudaMemsetAsync(&e->d_ctr->generated, 0, 8, e->stream));
-  const uint64_t n_states = hc.n_states;
-  collect_violations(e, hc);
-  if (e->verdict != TLAG_V_RUNNING && (e->m.flags & TLAG_F_KEEP_GOING)) {
-    // keep exploring: remember the first violation (lowest level, lowest index in it), clear the device slots
-    if (!e->kg_verdict) { e->kg_verdict = e->verdict; e->kg_detail = e->detail; e->kg_detail2 = e->detail2; e->kg_idx = e->viol_idx; }
-    e->verdict = TLAG_V_RUNNING;
-    const unsigned long long ones[4] = {~0ULL, ~0ULL, ~0ULL, ~0ULL};
-    CK(cudaMemcpyAsync(&e->d_ctr->viol_inv, ones, sizeof(ones), cudaMemcpyHostToDevice, e->stream));
-    CK(cudaStreamSynchronize(e->stream));
-  }
-  if (out) {
-    out->level = e->level; out->expanded = hi - lo; out->generated = gen_wave;
-    out->discovered = n_states - hi; out->distinct_total = n_states; out->generated_total = e->generated;
-    out->kernel_ms = ms;
-    out->retries = (uint32_t)attempt;
-  }
-  if (n_states > hi) e->depth = e->level + 1;
-  if (n_states > hi && e->verdict == TLAG_V_RUNNING) {
-    int rs = timed_cluster_slice(e, hi, n_states - hi, out);
-    if (rs) return rs;
-  }
-  {  // head-room for the next level: twice the observed discovered/expanded ratio, at least 4x
-    const double ratio = (double)(n_states - hi) / (double)(hi - lo);
-    e->growth_hint = ratio * 2.0 > 4.0 ? ratio * 2.0 : 4.0;
-  }
-  e->lo = hi; e->hi = n_states; e->level += 1;
-  if (e->verdict == TLAG_V_RUNNING && e->lo >= e->hi) {
-    e->verdict = e->kg_verdict ? e->kg_verdict : TLAG_V_OK;
-    if (e->kg_verdict) { e->detail = e->kg_detail; e->detail2 = e->kg_detail2; e->viol_idx = e->kg_idx; }
-  }
+  r = account_wave(e, hc, (e->m.flags & TLAG_F_KEEP_GOING) != 0, hi - lo, ms, out);
+  if (r) return r;
+  if (out) out->retries = (uint32_t)attempt;
+  r = close_level(e, hc.n_states, e->verdict == TLAG_V_RUNNING, out);
+  if (r) return r;
+  note_growth(e, hi - lo, e->hi - hi);
+  if (e->verdict == TLAG_V_RUNNING && e->lo >= e->hi) settle_verdict(e);
   if (out) out->verdict = e->verdict;
   return TLAG_OK;
 }
@@ -1360,7 +1389,7 @@ extern "C" int tlag_step(tlag_engine* e, tlag_wave_stats* out) {
 extern "C" int tlag_result_now(tlag_engine* e, tlag_result* out) {
   if (!e || !out) return TLAG_EINVAL;
   Counters hc;
-  CK(cudaMemcpy(&hc, e->d_ctr, sizeof(hc), cudaMemcpyDeviceToHost));
+  CK(read_counters(e, &hc));
   fill_result(e, out, hc.n_states);
   return TLAG_OK;
 }
@@ -1379,7 +1408,7 @@ extern "C" int tlag_run(tlag_engine* e, tlag_result* out) {
 extern "C" int tlag_read_states(tlag_engine* e, uint64_t first, uint64_t n, uint32_t* states_out) {
   if (!e || (!states_out && n)) return TLAG_EINVAL;
   Counters hc;
-  CK(cudaMemcpy(&hc, e->d_ctr, sizeof(hc), cudaMemcpyDeviceToHost));
+  CK(read_counters(e, &hc));
   if (first + n > hc.n_states) { e->err = "tlag_read_states: range beyond the state store"; return TLAG_EINVAL; }
   const uint64_t W = e->m.words_per_state;
   CK(cudaMemcpy(states_out, e->d_states + first * W, n * W * 4, cudaMemcpyDeviceToHost));
@@ -1389,7 +1418,7 @@ extern "C" int tlag_read_states(tlag_engine* e, uint64_t first, uint64_t n, uint
 extern "C" int tlag_digest(tlag_engine* e, uint64_t* xor_out, uint64_t* sum_out) {
   if (!e || !xor_out || !sum_out) return TLAG_EINVAL;
   Counters hc;
-  CK(cudaMemcpy(&hc, e->d_ctr, sizeof(hc), cudaMemcpyDeviceToHost));
+  CK(read_counters(e, &hc));
   if (!e->d_dig) CK(cudaMalloc(&e->d_dig, 16));
   unsigned long long* d2 = e->d_dig;
   CK(cudaMemsetAsync(d2, 0, 16, e->stream));
@@ -1405,45 +1434,10 @@ extern "C" int tlag_digest(tlag_engine* e, uint64_t* xor_out, uint64_t* sum_out)
   return TLAG_OK;
 }
 
-extern "C" int tlag_trace(tlag_engine* e, uint64_t state_idx, uint32_t* states_out, int32_t* actions_out, uint32_t* len_inout) {
-  if (!e || !len_inout) return TLAG_EINVAL;
-  Counters hc;
-  CK(cudaMemcpy(&hc, e->d_ctr, sizeof(hc), cudaMemcpyDeviceToHost));
-  if (state_idx >= hc.n_states) { e->err = "tlag_trace: no such state"; return TLAG_EINVAL; }
-  const uint64_t W = e->m.words_per_state;
-  std::vector<uint64_t> chain;
-  std::vector<int32_t> acts;
-  uint64_t cur = state_idx;
-  for (;;) {
-    uint32_t par = 0, meta = 0;
-    CK(cudaMemcpyAsync(&par, e->d_parent + cur, 4, cudaMemcpyDeviceToHost, e->stream));
-    CK(cudaMemcpyAsync(&meta, e->d_meta + cur, 4, cudaMemcpyDeviceToHost, e->stream));
-    CK(cudaStreamSynchronize(e->stream));
-    chain.push_back(cur);
-    acts.push_back(par == 0xFFFFFFFFu ? -1 : (int32_t)(meta >> 8));
-    if (par == 0xFFFFFFFFu) break;
-    cur = par;
-    if (chain.size() > (1u << 24)) { e->err = "tlag_trace: parent chain too long"; return TLAG_ESTATE; }
-  }
-  const uint32_t len = (uint32_t)chain.size();
-  if (len > *len_inout) { *len_inout = len; e->err = "tlag_trace: buffer too small"; return TLAG_EINVAL; }
-  for (uint32_t i = 0; i < len; ++i) {
-    const uint64_t s = chain[len - 1 - i];
-    if (states_out) CK(cudaMemcpy(states_out + (uint64_t)i * W, e->d_states + s * W, W * 4, cudaMemcpyDeviceToHost));
-    if (actions_out) actions_out[i] = acts[len - 1 - i];
-  }
-  *len_inout = len;
-  return TLAG_OK;
-}
-
-// One hop of a counterexample chain: the state at idx with its parent index and meta word (action id << 8 | rank that
-// expanded the parent).  With several ranks the parent lives in THAT rank's store: the host follows the chain across
-// ranks (tla_rust_b200/dist.py: counterexample).
-extern "C" int tlag_read_link(tlag_engine* e, uint64_t idx, uint32_t* state_out, uint32_t* parent_out, uint32_t* meta_out) {
-  if (!e || !parent_out || !meta_out) return TLAG_EINVAL;
-  Counters hc;
-  CK(cudaMemcpy(&hc, e->d_ctr, sizeof(hc), cudaMemcpyDeviceToHost));
-  if (idx >= hc.n_states) { e->err = "tlag_read_link: no such state"; return TLAG_EINVAL; }
+// One hop of a counterexample chain: the state at idx (when state_out) with its parent index and meta word (action id
+// << 8 | rank that expanded the parent).  With several ranks the parent lives in THAT rank's store: the host follows the
+// chain across ranks (tla_rust_b200/dist.py: counterexample).
+static int read_link(tlag_engine* e, uint64_t idx, uint32_t* state_out, uint32_t* parent_out, uint32_t* meta_out) {
   const uint64_t W = e->m.words_per_state;
   if (state_out) CK(cudaMemcpyAsync(state_out, e->d_states + idx * W, W * 4, cudaMemcpyDeviceToHost, e->stream));
   CK(cudaMemcpyAsync(parent_out, e->d_parent + idx, 4, cudaMemcpyDeviceToHost, e->stream));
@@ -1452,10 +1446,48 @@ extern "C" int tlag_read_link(tlag_engine* e, uint64_t idx, uint32_t* state_out,
   return TLAG_OK;
 }
 
+extern "C" int tlag_trace(tlag_engine* e, uint64_t state_idx, uint32_t* states_out, int32_t* actions_out, uint32_t* len_inout) {
+  if (!e || !len_inout) return TLAG_EINVAL;
+  Counters hc;
+  CK(read_counters(e, &hc));
+  if (state_idx >= hc.n_states) { e->err = "tlag_trace: no such state"; return TLAG_EINVAL; }
+  const uint64_t W = e->m.words_per_state;
+  std::vector<uint32_t> words;   // the chain's states from state_idx back, while they fit the caller's buffer
+  std::vector<int32_t> acts;
+  uint64_t cur = state_idx;
+  for (;;) {
+    uint32_t par = 0, meta = 0;
+    const bool keep = states_out && acts.size() < *len_inout;
+    if (keep) words.resize(words.size() + W);
+    int r = read_link(e, cur, keep ? words.data() + words.size() - W : nullptr, &par, &meta);
+    if (r) return r;
+    acts.push_back(par == 0xFFFFFFFFu ? -1 : (int32_t)(meta >> 8));
+    if (par == 0xFFFFFFFFu) break;
+    cur = par;
+    if (acts.size() > (1u << 24)) { e->err = "tlag_trace: parent chain too long"; return TLAG_ESTATE; }
+  }
+  const uint32_t len = (uint32_t)acts.size();
+  if (len > *len_inout) { *len_inout = len; e->err = "tlag_trace: buffer too small"; return TLAG_EINVAL; }
+  for (uint32_t i = 0; i < len; ++i) {
+    if (states_out) memcpy(states_out + (uint64_t)i * W, words.data() + (uint64_t)(len - 1 - i) * W, W * 4);
+    if (actions_out) actions_out[i] = acts[len - 1 - i];
+  }
+  *len_inout = len;
+  return TLAG_OK;
+}
+
+extern "C" int tlag_read_link(tlag_engine* e, uint64_t idx, uint32_t* state_out, uint32_t* parent_out, uint32_t* meta_out) {
+  if (!e || !parent_out || !meta_out) return TLAG_EINVAL;
+  Counters hc;
+  CK(read_counters(e, &hc));
+  if (idx >= hc.n_states) { e->err = "tlag_read_link: no such state"; return TLAG_EINVAL; }
+  return read_link(e, idx, state_out, parent_out, meta_out);
+}
+
 // ---- multi-GPU building blocks -----------------------------------------------------
 extern "C" int tlag_frontier(tlag_engine* e, uint64_t* first_idx, uint64_t* count) {
   if (!e) return TLAG_EINVAL;
-  if (e->level == 0) { e->level = 1; e->lo = 0; e->depth = e->hi > 0 ? 1 : 0; }
+  start_search(e);
   if (first_idx) *first_idx = e->lo;
   if (count) *count = e->hi - e->lo;
   return TLAG_OK;
@@ -1482,7 +1514,7 @@ extern "C" int tlag_expand_route(tlag_engine* e, uint32_t n_ranks, uint64_t firs
                                  uint64_t cap_records, uint64_t* counts, tlag_wave_stats* out) {
   if (!e || !counts || n_ranks == 0 || n_ranks > 16) return TLAG_EINVAL;
   if (out) memset(out, 0, sizeof(*out));
-  if (e->level == 0) { e->level = 1; e->lo = 0; e->depth = 1; }
+  start_search(e);
   uint64_t lo = e->lo + first, hi = lo + count;
   if (lo > e->hi) lo = e->hi;
   if (hi > e->hi) hi = e->hi;
@@ -1498,17 +1530,10 @@ extern "C" int tlag_expand_route(tlag_engine* e, uint32_t n_ranks, uint64_t firs
   CK(cudaMemsetAsync(e->d_ctr->send_count, 0, sizeof(unsigned long long) * 16, e->stream));
   CK(cudaMemsetAsync(&e->d_ctr->route_overflow, 0, 8, e->stream));   // a failed attempt may be retried with
   CK(cudaMemsetAsync(&e->d_ctr->generated, 0, 8, e->stream));        // larger regions: start from clean counters
-  CK(cudaEventRecord(e->ev0, e->stream));
-  if (hi > lo) {
-    cudaError_t ce = launch_wave<1>(e, lo, hi);
-    if (ce != cudaSuccess) { e->err = std::string("k_wave<route> launch: ") + cudaGetErrorString(ce); return TLAG_ECUDA; }
-  }
-  CK(cudaEventRecord(e->ev1, e->stream));
   Counters hc;
-  CK(cudaMemcpyAsync(&hc, e->d_ctr, sizeof(hc), cudaMemcpyDeviceToHost, e->stream));
-  CK(cudaStreamSynchronize(e->stream));
   float ms = 0;
-  CK(cudaEventElapsedTime(&ms, e->ev0, e->ev1));
+  r = timed(e, &ms, &hc, [&] { if (hi > lo) CK(launch_wave<1>(e, lo, hi)); return TLAG_OK; });
+  if (r) return r;
   e->dev_seconds += ms * 1e-3;
   if (hc.route_overflow) {
     // The caller re-runs this chunk with larger regions and throws this attempt's buffer away -- including the records
@@ -1519,42 +1544,30 @@ extern "C" int tlag_expand_route(tlag_engine* e, uint32_t n_ranks, uint64_t firs
     e->err = "send buffer overflow in tlag_expand_route";
     return TLAG_EOVERFLOW;
   }
-  e->generated += hc.generated;
-  CK(cudaMemsetAsync(&e->d_ctr->generated, 0, 8, e->stream));
-  for (uint32_t r = 0; r < n_ranks; ++r) counts[r] = hc.send_count[r];
-  collect_violations(e, hc);
-  if (out) {
-    out->level = e->level; out->expanded = hi - lo; out->generated = hc.generated;
-    out->distinct_total = hc.n_states; out->generated_total = e->generated; out->kernel_ms = ms;
-    out->verdict = e->verdict;
-  }
-  return TLAG_OK;
+  for (uint32_t k = 0; k < n_ranks; ++k) counts[k] = hc.send_count[k];
+  return account_wave(e, hc, false, hi - lo, ms, out);
 }
 
 extern "C" int tlag_insert_records(tlag_engine* e, uint64_t d_recv, uint64_t n_records, uint32_t, uint64_t* n_new) {
   if (!e) return TLAG_EINVAL;
   Counters hc;
-  CK(cudaMemcpyAsync(&hc, e->d_ctr, sizeof(hc), cudaMemcpyDeviceToHost, e->stream));
-  CK(cudaStreamSynchronize(e->stream));
+  CK(read_counters(e, &hc));
   const uint64_t before = hc.n_states;
-  int r = grow_store_if_needed(e, before + n_records + 1024);
-  if (r) return r;
-  r = grow_table_if_needed(e, before + n_records);
+  int r = reserve_level(e, before + n_records + 1024, before + n_records);
   if (r) return r;
   if (n_records) {
-    CK(cudaEventRecord(e->ev0, e->stream));
-    k_insert_records<<<(unsigned)((n_records + 255) / 256), 256, 0, e->stream>>>(e->p, (const uint32_t*)(uintptr_t)d_recv, n_records);
-    e->launches++;
-    CK(cudaGetLastError());
-    CK(cudaEventRecord(e->ev1, e->stream));
-    CK(cudaEventSynchronize(e->ev1));
     float ms = 0;
-    CK(cudaEventElapsedTime(&ms, e->ev0, e->ev1));
+    r = timed(e, &ms, &hc, [&] {
+      k_insert_records<<<(unsigned)((n_records + 255) / 256), 256, 0, e->stream>>>(e->p, (const uint32_t*)(uintptr_t)d_recv, n_records);
+      e->launches++;
+      CK(cudaGetLastError());
+      return TLAG_OK;
+    });
+    if (r) return r;
     e->dev_seconds += ms * 1e-3;
   }
-  CK(cudaMemcpy(&hc, e->d_ctr, sizeof(hc), cudaMemcpyDeviceToHost));
-  if (hc.store_overflow) { e->err = "state store overflow: raise max_states"; return TLAG_ENOMEM; }
-  if (hc.table_full) { e->err = "seen-set table full"; return TLAG_ENOMEM; }
+  r = overflow_error(e, hc, "state store overflow: raise max_states", "seen-set table full");
+  if (r) return r;
   if (n_new) *n_new = hc.n_states - before;
   return TLAG_OK;
 }
@@ -1640,18 +1653,16 @@ extern "C" int tlag_p2p_level(tlag_engine* e, uint64_t n_chunks, uint64_t chunk_
   if (!e || chunk_states == 0) return TLAG_EINVAL;
   if (!e->p2p_ready && e->q.n_ranks > 1) { e->err = "tlag_p2p_level before every peer was attached"; return TLAG_ESTATE; }
   if (out) memset(out, 0, sizeof(*out));
-  if (e->level == 0) { e->level = 1; e->lo = 0; e->depth = e->hi > 0 ? 1 : 0; }
+  start_search(e);
   const uint32_t n_ranks = (uint32_t)e->q.n_ranks;
   // room for what may arrive this level (the caller passes the all-reduced estimate; at least the heuristic)
   uint64_t expect = (uint64_t)((double)(e->hi - e->lo) * e->growth_hint) + 4096;
   if (expect_inbound > expect) expect = expect_inbound;
   Counters hc;
-  CK(cudaMemcpy(&hc, e->d_ctr, sizeof(hc), cudaMemcpyDeviceToHost));
+  CK(read_counters(e, &hc));
   const uint64_t before = hc.n_states;
   e->p2p_level_start = before; e->p2p_level_generated = 0;
-  int r = grow_store_if_needed(e, before + expect);
-  if (r) return r;
-  r = grow_table_if_needed(e, before + expect);
+  int r = reserve_level(e, before + expect, before + expect);
   if (r) return r;
   e->p.n_ranks = (int)n_ranks; e->p.rank = e->q.rank;
   r = ensure_sent_cache(e);
@@ -1660,46 +1671,34 @@ extern "C" int tlag_p2p_level(tlag_engine* e, uint64_t n_chunks, uint64_t chunk_
   e->p.region_cap = e->q.region_cap;
   CK(cudaMemsetAsync(&e->d_ctr->route_overflow, 0, 8, e->stream));
   CK(cudaMemsetAsync(&e->d_ctr->generated, 0, 8, e->stream));
-  CK(cudaEventRecord(e->ev0, e->stream));
   const unsigned push_blocks = 64, ins_blocks = (unsigned)e->sm_count * 4;
-  for (uint64_t c = 0; c < n_chunks; ++c) {
-    const unsigned long long seq = ++e->p2p_seq;
-    uint64_t lo = e->lo + c * chunk_states, hi = lo + chunk_states;
-    if (lo > e->hi) lo = e->hi;
-    if (hi > e->hi) hi = e->hi;
-    CK(cudaMemsetAsync(&e->d_ctr->work, 0, 8, e->stream));
-    CK(cudaMemsetAsync(e->d_ctr->send_count, 0, sizeof(unsigned long long) * 16, e->stream));
-    if (hi > lo) {
-      cudaError_t ce = launch_wave<1>(e, lo, hi);
-      if (ce != cudaSuccess) { e->err = std::string("route wave launch: ") + cudaGetErrorString(ce); return TLAG_ECUDA; }
-    }
-    k_push<<<dim3(push_blocks, n_ranks), 256, 0, e->stream>>>(e->q, e->d_ctr, seq);
-    k_insert_inbox<<<ins_blocks, 256, 0, e->stream>>>(e->p, e->q, seq);
-    e->launches += 2;
-    CK(cudaGetLastError());
-  }
-  CK(cudaEventRecord(e->ev1, e->stream));
-  CK(cudaMemcpyAsync(&hc, e->d_ctr, sizeof(hc), cudaMemcpyDeviceToHost, e->stream));
-  CK(cudaStreamSynchronize(e->stream));
   float ms = 0;
-  CK(cudaEventElapsedTime(&ms, e->ev0, e->ev1));
+  r = timed(e, &ms, &hc, [&] {
+    for (uint64_t c = 0; c < n_chunks; ++c) {
+      const unsigned long long seq = ++e->p2p_seq;
+      uint64_t lo = e->lo + c * chunk_states, hi = lo + chunk_states;
+      if (lo > e->hi) lo = e->hi;
+      if (hi > e->hi) hi = e->hi;
+      CK(cudaMemsetAsync(&e->d_ctr->work, 0, 8, e->stream));
+      CK(cudaMemsetAsync(e->d_ctr->send_count, 0, sizeof(unsigned long long) * 16, e->stream));
+      if (hi > lo) CK(launch_wave<1>(e, lo, hi));
+      k_push<<<dim3(push_blocks, n_ranks), 256, 0, e->stream>>>(e->q, e->d_ctr, seq);
+      k_insert_inbox<<<ins_blocks, 256, 0, e->stream>>>(e->p, e->q, seq);
+      e->launches += 2;
+      CK(cudaGetLastError());
+    }
+    return TLAG_OK;
+  });
+  if (r) return r;
   e->dev_seconds += ms * 1e-3;
   if (hc.route_overflow) { e->err = "send region overflow in tlag_p2p_level: use smaller chunks or larger regions"; return TLAG_EOVERFLOW; }
-  if (hc.store_overflow) { e->err = "state store overflow in tlag_p2p_level"; return TLAG_ENOMEM; }
-  if (hc.table_full) { e->err = "seen-set table full in tlag_p2p_level"; return TLAG_ENOMEM; }
-  e->generated += hc.generated;
+  r = overflow_error(e, hc, "state store overflow in tlag_p2p_level", "seen-set table full in tlag_p2p_level");
+  if (r) return r;
   e->p2p_level_generated = hc.generated;
-  CK(cudaMemsetAsync(&e->d_ctr->generated, 0, 8, e->stream));
-  collect_violations(e, hc);
-  if (out) {
-    out->level = e->level; out->expanded = e->hi - e->lo; out->generated = hc.generated;
-    out->discovered = hc.n_states - before; out->distinct_total = hc.n_states; out->generated_total = e->generated;
-    out->kernel_ms = ms; out->verdict = e->verdict;
-  }
-  {
-    const double ratio = (double)(hc.n_states - before) / (double)((e->hi - e->lo) ? (e->hi - e->lo) : 1);
-    e->growth_hint = ratio * 2.0 > 4.0 ? ratio * 2.0 : 4.0;
-  }
+  r = account_wave(e, hc, false, e->hi - e->lo, ms, out);
+  if (r) return r;
+  if (out) out->discovered = hc.n_states - before;
+  note_growth(e, e->hi - e->lo, hc.n_states - before);
   return TLAG_OK;
 }
 
@@ -1708,11 +1707,9 @@ extern "C" int tlag_p2p_level(tlag_engine* e, uint64_t n_chunks, uint64_t chunk_
 // from the store, the routed-fingerprint cache is emptied; the inbox chunk numbering simply continues.
 extern "C" int tlag_p2p_rollback(tlag_engine* e) {
   if (!e || !e->d_p2p) return TLAG_EINVAL;
-  CK(cudaStreamSynchronize(e->stream));
   int r = rollback_wave(e, e->p2p_level_start, e->p2p_level_start + 4096);
   if (r) return r;
   if (e->d_sent) CK(cudaMemsetAsync(e->d_sent, 0, (e->p.sent_mask + 1) * 8, e->stream));
-  CK(cudaMemsetAsync(&e->d_ctr->route_overflow, 0, 8, e->stream));
   CK(cudaStreamSynchronize(e->stream));
   e->generated -= e->p2p_level_generated;
   e->p2p_level_generated = 0;
@@ -1722,15 +1719,8 @@ extern "C" int tlag_p2p_rollback(tlag_engine* e) {
 
 extern "C" int tlag_advance_level(tlag_engine* e, tlag_wave_stats* out) {
   if (!e) return TLAG_EINVAL;
+  if (out) memset(out, 0, sizeof(*out));
   Counters hc;
-  CK(cudaMemcpy(&hc, e->d_ctr, sizeof(hc), cudaMemcpyDeviceToHost));
-  const uint64_t n_states = hc.n_states;
-  if (out) { memset(out, 0, sizeof(*out)); out->level = e->level; out->discovered = n_states - e->hi; out->distinct_total = n_states; out->generated_total = e->generated; out->verdict = e->verdict; }
-  if (n_states > e->hi) {
-    e->depth = e->level + 1;
-    int rs = timed_cluster_slice(e, e->hi, n_states - e->hi, out);
-    if (rs) return rs;
-  }
-  e->lo = e->hi; e->hi = n_states; e->level += 1;
-  return TLAG_OK;
+  CK(read_counters(e, &hc));
+  return close_level(e, hc.n_states, true, out);
 }
