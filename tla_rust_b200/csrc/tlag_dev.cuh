@@ -31,7 +31,13 @@ struct DevParams {
   uint32_t n_off, p_off;
   int W;
   uint32_t* states; uint32_t* parent; uint32_t* meta;
-  unsigned long long cap_states;
+  unsigned long long cap_states;    // append limit: a row at or past it is counted in n_states, not written
+  // Where appended rows go: row pos's W words at app + pos * app_stride, its parent and meta words at app_parent and
+  // app_meta + pos * pm_stride.  That is the store (strides W and 1), or while a level is discovered its discovery
+  // buffer of records [W words, parent, meta] (both strides W + 2), which the host clusters into the store when the level
+  // ends.  For the buffer the host offsets the pointers by the level's first row, so that appends take no branch.
+  uint32_t* app; uint32_t* app_parent; uint32_t* app_meta;
+  unsigned app_stride, pm_stride;
   unsigned long long* table; unsigned long long mask;
   Counters* ctr;
   uint32_t flags;
@@ -123,6 +129,12 @@ __device__ __forceinline__ unsigned lanemask_lt() {
 // parent index points into)
 __device__ __forceinline__ uint32_t tlag_meta(int aid, int rank) { return ((uint32_t)aid << 8) | (uint32_t)(rank & 0xFF); }
 
+// Where new row pos (< cap_states) is written: its W words, its parent and its meta word (DevParams::app)
+struct RowDst { uint32_t* w; uint32_t* parent; uint32_t* meta; };
+__device__ __forceinline__ RowDst row_dst(const DevParams& p, unsigned long long pos) {
+  return {p.app + pos * p.app_stride, p.app_parent + pos * p.pm_stride, p.app_meta + pos * p.pm_stride};
+}
+
 // Appends a new state to the tail of the store.  Only the lanes of `group` call it, each with a new state: one tail
 // atomic for the group, rows in lane order.  A row past cap_states is still counted in n_states (the host sizes the
 // rerun of the level from it) and is reported in store_overflow.
@@ -134,10 +146,10 @@ __device__ __forceinline__ void store_append(const DevParams& p, unsigned group,
   base = __shfl_sync(group, base, leader);
   const unsigned long long pos = base + (unsigned long long)__popc(group & lanemask_lt());
   if (pos < p.cap_states) {
-    uint32_t* dst = p.states + pos * (unsigned long long)W;
-    for (int i = 0; i < W; ++i) dst[i] = w[i];
-    p.parent[pos] = parent;
-    p.meta[pos] = meta;
+    const RowDst d = row_dst(p, pos);
+    for (int i = 0; i < W; ++i) d.w[i] = w[i];
+    *d.parent = parent;
+    *d.meta = meta;
   } else {
     atomicExch(&p.ctr->store_overflow, 1ULL);
   }

@@ -48,7 +48,7 @@ static __device__ __noinline__ void sl_emit_frame(tlag_sl_cx* cx, const int32_t*
 
 #ifdef TLAG_SL_STAGED
 // The whole warp: fingerprint the staged successors and probe the seen-set for them, then append the new ones to the
-// store as one contiguous run (one tail atomic, coalesced stores).  Semantics as sl_emit_words: a row past the store's
+// store (its discovery buffer while the level has one) as one contiguous run (one tail atomic, coalesced stores).  Semantics as sl_emit_words: a row past the store's
 // capacity is counted in n_states and reported as an overflow, a full table as table_full.
 static __device__ __forceinline__ void sl_flush(const DevParams& p, unsigned cap) {
   constexpr int W = TLAG_SL_W, R = TLAG_SL_STAGE_SLOTS / 32;
@@ -85,14 +85,15 @@ static __device__ __forceinline__ void sl_flush(const DevParams& p, unsigned cap
     for (unsigned t = lane; t < total * W; t += 32) {
       const unsigned row = t / W, k = t - row * W;
       const unsigned long long pos = base + row;
-      if (pos < p.cap_states) p.states[pos * W + k] = tlag_sl_stage[warp][k][tlag_sl_row[warp][row]];
+      if (pos < p.cap_states) row_dst(p, pos).w[k] = tlag_sl_stage[warp][k][tlag_sl_row[warp][row]];
     }
     for (unsigned row = lane; row < total; row += 32) {
       const unsigned long long pos = base + row;
       const unsigned s = tlag_sl_row[warp][row];
       if (pos < p.cap_states) {
-        p.parent[pos] = tlag_sl_stage[warp][W][s];
-        p.meta[pos] = tlag_sl_stage[warp][W + 1][s];
+        const RowDst d = row_dst(p, pos);
+        *d.parent = tlag_sl_stage[warp][W][s];
+        *d.meta = tlag_sl_stage[warp][W + 1][s];
       } else {
         atomicExch(&p.ctr->store_overflow, 1ULL);
       }

@@ -75,8 +75,12 @@ struct tlag_engine {
   bool restarting = false;
   bool tight = false;               // TLAG_TIGHT_HEADROOM (test hook): store and table sized for no growth, see tlag_create
   double growth_hint = 4.0;
-  void* d_sort = nullptr; uint64_t sort_bytes = 0;
-  // clustering pass: the rank set ([RankSetCtl | 2^log2 keys | 2^log2 ranks]), its size carried from level to level
+  double disc_hint = 4.0;           // discovery buffer rows per state expanded, for the next level (note_growth)
+  // discovery buffer: the open level's new rows (DevParams::disc), put into the store by close_level
+  void* d_disc = nullptr; uint64_t disc_bytes = 0; bool disc_open = false;
+  void* d_sort = nullptr; uint64_t sort_bytes = 0;    // clustering pass: (rank, index) pairs, double-buffered, CUB temp
+  // clustering pass: the rank set ([RankSetCtl | keys | ranks | key lists], cluster_slice), its size carried from level to
+  // level
   void* d_rset = nullptr; uint64_t rset_bytes = 0; unsigned rset_log2 = 16; bool rset_fixed = false;
   unsigned long long* d_sent = nullptr;
   uint8_t* d_succ = nullptr; uint64_t succ_cap = 0;   // sliced build: per-frontier-state "has a successor" flags
@@ -443,86 +447,65 @@ __global__ void k_digest(DevParams p, unsigned long long n, unsigned long long* 
 // (mean path length) / (union length).  States that agree on the tail of the packed vector (the last
 // variables, for the Paxos models the high bits of the msgs bitset) follow similar paths: measured on
 // a 4096-state window of MCPaxos3_b3 level 14, lane utilisation is 0.35 in discovery order, 0.31 in random
-// order and 0.54 when sorted by the last packed word.  Each newly discovered level slice is therefore
-// reordered (stable data: nothing references those indices yet) by a 64-bit key of its last two words,
-// key = w[W-1] << 32 | w[W-2], stably, so equal keys keep their discovery order.
+// order and 0.54 when sorted by the last packed word.  Each newly discovered level is therefore reordered by a
+// 64-bit key of its last two words, key = w[W-1] << 32 | w[W-2], stably, so equal keys keep their discovery order
+// (an unstable order within a key costs the next wave time: 8 - 10 % on MCssi_4x3, 1 % on MCPaxos3_b4).
 //
-// A level holds few distinct keys (MCPaxos3_b4: 1 K - 100 K in levels of up to millions of states; Raft and SSI a few
-// hundred), so the slice is sorted on the key's dense rank among the level's distinct keys, not on the key itself: the
-// same permutation, on 32-bit keys of ceil(log2(distinct)) bits -- 2 or 3 radix passes instead of 8 passes over 64-bit
-// keys.  The pass:
-//   k_cluster_pack    copies the slice's rows, parents and meta words out of the store into records of W + 2 words
-//                     (one contiguous read per record later) and writes each state's key;
-//   k_rset_insert     puts the keys into a small open-addressed set (the rank set, L2-resident at these sizes);
-//   k_rset_list, a sort of the distinct keys, k_rset_rank   give every distinct key its rank;
-//   k_rank_states     writes each state's rank, then a stable radix sort of (rank, index) over the rank's bits;
+// A level's new rows are appended to a discovery buffer of records [W words, parent, meta] (DevParams::app), and the
+// pass moves each record once, straight to its final row in the store.  A level holds few distinct keys (MCPaxos3_b4:
+// 1 K - 100 K in levels of up to millions of states; Raft and SSI a few hundred), so the level is sorted on the key's
+// dense rank among the level's distinct keys, not on the key itself: the same permutation, on 32-bit keys of
+// ceil(log2(distinct)) bits -- 2 or 3 radix passes instead of 8 passes over 64-bit keys.  The pass:
+//   k_rset_insert     puts each record's key into a small open-addressed set (the rank set, L2-resident at these sizes)
+//                     and writes the key's slot;
+//   k_rset_list, a sort of the distinct keys, k_rset_rank   give every slot its key's rank;
+//   k_rank_states     turns each record's slot into its rank and writes its index, then a stable radix sort of
+//                     (rank, index) over the rank's bits;
 //   k_cluster_gather  writes record idx[i] to store row first + i, a warp per 32 rows, stores coalesced.
 #define TLAG_RSET_EMPTY 0xFFFFFFFFFFFFFFFFull   /* empty slot; a key equal to it is counted aside (it is the largest) */
 struct RankSetCtl { unsigned n, full, has_max, n_list; };
-#define TLAG_CLUSTER_ILP 4   /* words each lane loads before it stores them (pack, gather): latency-bound otherwise */
+#define TLAG_CLUSTER_ILP 4   /* words each lane loads before it stores them (gather): latency-bound otherwise */
 
 __device__ __forceinline__ unsigned long long rset_hash(unsigned long long k) {   // splitmix64 finaliser
   k ^= k >> 30; k *= 0xbf58476d1ce4e5b9ull; k ^= k >> 27; k *= 0x94d049bb133111ebull; return k ^ (k >> 31);
 }
 
-__global__ void k_cluster_pack(const uint32_t* __restrict__ st, const uint32_t* __restrict__ parent,
-                               const uint32_t* __restrict__ meta, unsigned long long n, int W,
-                               uint32_t* __restrict__ rec, unsigned long long* __restrict__ keys) {
-  const unsigned lane = threadIdx.x & 31;
-  const unsigned long long r0 = ((unsigned long long)blockIdx.x * blockDim.x + threadIdx.x) & ~31ull;
-  if (r0 >= n) return;
-  const unsigned rows = n - r0 < 32 ? (unsigned)(n - r0) : 32u;
-  const uint32_t* src = st + r0 * (unsigned long long)W;
-  uint32_t* dst = rec + r0 * (unsigned long long)(W + 2);
-  const unsigned long long i = r0 + lane;
-  const uint32_t par = lane < rows ? __ldcs(parent + i) : 0, met = lane < rows ? __ldcs(meta + i) : 0;
-  const unsigned words = rows * (unsigned)W;
-  for (unsigned base = 0; base < words; base += 32 * TLAG_CLUSTER_ILP) {   // several loads in flight per lane
-    uint32_t v[TLAG_CLUSTER_ILP];
-#pragma unroll
-    for (int u = 0; u < TLAG_CLUSTER_ILP; ++u) {
-      const unsigned k = base + u * 32 + lane;
-      v[u] = k < words ? src[k] : 0;
-    }
-#pragma unroll
-    for (int u = 0; u < TLAG_CLUSTER_ILP; ++u) {
-      const unsigned k = base + u * 32 + lane, r = k / (unsigned)W, c = k - r * (unsigned)W;
-      if (k < words) dst[r * (W + 2) + c] = v[u];
-    }
-  }
-  if (lane < rows) {
-    dst[lane * (W + 2) + W] = par;
-    dst[lane * (W + 2) + W + 1] = met;
-    const uint32_t* s = src + lane * (unsigned long long)W;
-    const unsigned long long hi = s[W - 1], lo = W >= 2 ? s[W - 2] : 0;
-    keys[i] = (hi << 32) | lo;
-  }
-}
-
-__global__ void k_rset_insert(const unsigned long long* __restrict__ keys, unsigned long long n,
-                              unsigned long long* __restrict__ table, unsigned long long mask, RankSetCtl* ctl) {
-  const unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  const unsigned long long key = __ldcs(keys + i);
-  // lanes of a warp often share a key (successors of like states): one lane per distinct key probes the set
-  const unsigned peers = __match_any_sync(__activemask(), key);
-  if ((threadIdx.x & 31) != (unsigned)(__ffs(peers) - 1)) return;
-  if (key == TLAG_RSET_EMPTY) { if (!*(volatile unsigned*)&ctl->has_max) ctl->has_max = 1; return; }
+// The slot of `key` in the rank set (mask + 1 slots; slot mask + 1 for the TLAG_RSET_EMPTY key), inserted if absent; a
+// set past half full (or full) is flagged for the host to grow and refill.
+__device__ __forceinline__ unsigned long long rset_slot(unsigned long long* table, unsigned long long mask, RankSetCtl* ctl,
+                                                        unsigned long long key) {
+  if (key == TLAG_RSET_EMPTY) { if (!*(volatile unsigned*)&ctl->has_max) ctl->has_max = 1; return mask + 1; }
   unsigned long long h = rset_hash(key) & mask;
   for (unsigned long long probes = 0; probes <= mask; ++probes, h = (h + 1) & mask) {
     unsigned long long v = __ldcg(table + h);
-    if (v == key) return;
+    if (v == key) return h;
     if (v == TLAG_RSET_EMPTY) {
-      if (*(volatile unsigned*)&ctl->full) return;
+      if (*(volatile unsigned*)&ctl->full) return 0;
       v = atomicCAS(table + h, TLAG_RSET_EMPTY, key);
-      if (v == TLAG_RSET_EMPTY) {                 // new distinct key; past half the slots the set is grown and refilled
+      if (v == TLAG_RSET_EMPTY) {                 // new distinct key
         if ((unsigned long long)atomicAdd(&ctl->n, 1u) + 1 > (mask + 1) / 2) ctl->full = 1;
-        return;
+        return h;
       }
-      if (v == key) return;
+      if (v == key) return h;
     }
   }
   ctl->full = 1;
+  return 0;
+}
+
+// record i of the discovery buffer -> its key's slot; the key is the record's words W-1, W-2 (next to parent and meta)
+__global__ void k_rset_insert(const uint32_t* __restrict__ rec, unsigned long long n, int W, unsigned long long* table,
+                              unsigned long long mask, RankSetCtl* ctl, uint32_t* __restrict__ slot_of) {
+  const unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const uint32_t* r = rec + i * (unsigned long long)(W + 2);
+  const unsigned long long key = ((unsigned long long)r[W - 1] << 32) | (W >= 2 ? r[W - 2] : 0u);
+  // lanes of a warp often share a key (successors of like states): one lane per distinct key probes the set
+  const unsigned peers = __match_any_sync(__activemask(), key);
+  const int leader = __ffs(peers) - 1;
+  unsigned long long h = 0;
+  if ((int)(threadIdx.x & 31) == leader) h = rset_slot(table, mask, ctl, key);
+  slot_of[i] = (uint32_t)__shfl_sync(peers, h, leader);
 }
 
 __global__ void k_rset_list(const unsigned long long* __restrict__ table, unsigned long long slots,
@@ -540,28 +523,33 @@ __device__ __forceinline__ unsigned long long rset_find(const unsigned long long
   return h;
 }
 
-// sorted[r] = the distinct key of rank r
+// sorted[r] = the distinct key of rank r (r < n); the TLAG_RSET_EMPTY key, the largest, has rank n (slot mask + 1)
 __global__ void k_rset_rank(const unsigned long long* __restrict__ sorted, unsigned n,
                             const unsigned long long* __restrict__ table, unsigned long long mask, uint32_t* __restrict__ rank) {
   const unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) rank[rset_find(table, mask, sorted[i])] = i;
+  else if (i == n) rank[mask + 1] = n;
 }
 
-__global__ void k_rank_states(const unsigned long long* __restrict__ keys, unsigned long long n,
-                              const unsigned long long* __restrict__ table, unsigned long long mask,
-                              const uint32_t* __restrict__ rank, uint32_t max_rank,
-                              uint32_t* __restrict__ r_out, uint32_t* __restrict__ idx) {
+// Entry i of the sort: the rank of record j and j itself, j = i (rank_out may be `slot`: each thread reads its own
+// entry before it writes it).  chunk_order: in every full window of 64 chunks of 32 records the chunks enter in reverse
+// order (TLAG_CLUSTER_CHUNK_ORDER, cluster_slice).
+__global__ void k_rank_states(const uint32_t* slot, unsigned long long n, const uint32_t* __restrict__ rank,
+                              uint32_t* rank_out, uint32_t* __restrict__ idx, int chunk_order) {
   const unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  const unsigned long long key = __ldcs(keys + i);
-  const unsigned peers = __match_any_sync(__activemask(), key);    // one lookup per distinct key of the warp
-  const int leader = __ffs(peers) - 1;
-  uint32_t rk = 0;
-  if ((int)(threadIdx.x & 31) == leader) rk = key == TLAG_RSET_EMPTY ? max_rank : rank[rset_find(table, mask, key)];
-  r_out[i] = __shfl_sync(peers, rk, leader);
-  idx[i] = (uint32_t)i;
+  unsigned long long j = i;
+  if (chunk_order) {
+    const unsigned long long c = i >> 5, w = c & ~63ull;
+    if ((w + 64) * 32 <= n) j = ((w | (63 - (c & 63))) << 5) | (i & 31);
+  }
+  const uint32_t r = __ldg(rank + slot[j]);
+  rank_out[i] = r;
+  idx[i] = (uint32_t)j;
 }
 
+// Store row first + i <- record idx[i] of the discovery buffer (st, parent and meta point at row first; without idx,
+// record i: discovery order).  A warp writes 32 consecutive rows: coalesced stores.
 __global__ void k_cluster_gather(const uint32_t* __restrict__ rec, const uint32_t* __restrict__ idx,
                                  unsigned long long n, int W, uint32_t* __restrict__ st,
                                  uint32_t* __restrict__ parent, uint32_t* __restrict__ meta) {
@@ -569,7 +557,7 @@ __global__ void k_cluster_gather(const uint32_t* __restrict__ rec, const uint32_
   const unsigned long long r0 = ((unsigned long long)blockIdx.x * blockDim.x + threadIdx.x) & ~31ull;
   if (r0 >= n) return;
   const unsigned rows = n - r0 < 32 ? (unsigned)(n - r0) : 32u;
-  const unsigned long long j = lane < rows ? __ldcs(idx + r0 + lane) : 0;
+  const unsigned long long j = lane < rows ? (idx ? (unsigned long long)__ldcs(idx + r0 + lane) : r0 + lane) : 0;
   const uint32_t* mine = rec + j * (unsigned long long)(W + 2);
   const uint32_t par = lane < rows ? mine[W] : 0, met = lane < rows ? mine[W + 1] : 0;
   uint32_t* dst = st + r0 * (unsigned long long)W;
@@ -634,11 +622,11 @@ static void trim_pool(tlag_engine* e) {
   if (cudaDeviceGetDefaultMemPool(&pool, e->m.device) == cudaSuccess) cudaMemPoolTrimTo(pool, 0);
   cudaGetLastError();
 }
-static cudaError_t dmalloc(tlag_engine* e, void* pp, size_t bytes) {
+static cudaError_t dmalloc(tlag_engine* e, void* pp, size_t bytes, bool trim = true) {
   static const bool plain = getenv("TLAG_NO_POOL") != nullptr;
   if (plain) return cudaMalloc((void**)pp, bytes);
   cudaError_t r = cudaMallocAsync((void**)pp, bytes, e->stream);
-  if (r == cudaErrorMemoryAllocation) {
+  if (r == cudaErrorMemoryAllocation && trim) {
     cudaGetLastError();
     trim_pool(e);
     r = cudaMallocAsync((void**)pp, bytes, e->stream);
@@ -651,6 +639,21 @@ static void dfree(tlag_engine* e, void* p) {
   if (plain) cudaFree(p); else cudaFreeAsync(p, e->stream);
 }
 
+// DevParams::app at the store, or with the level open at its discovery buffer (row hi = record 0).  The store's append
+// limit is its capacity; an open level's is set by open_level.
+static void point_appends(tlag_engine* e) {
+  DevParams& p = e->p;
+  const unsigned W = (unsigned)e->m.words_per_state;
+  if (e->disc_open) {
+    const uintptr_t row0 = (uintptr_t)e->d_disc - (uintptr_t)(e->hi * (W + 2) * 4);   // never dereferenced below row hi
+    p.app = (uint32_t*)row0; p.app_parent = (uint32_t*)(row0 + W * 4); p.app_meta = (uint32_t*)(row0 + (W + 1) * 4);
+    p.app_stride = p.pm_stride = W + 2;
+  } else {
+    p.app = p.states; p.app_parent = p.parent; p.app_meta = p.meta;
+    p.app_stride = W; p.pm_stride = 1;
+    p.cap_states = e->cap_states;
+  }
+}
 
 static const int kFrameClasses[] = {64, 128, 256, 512, 1024, 2048, 4096, 8192};
 
@@ -781,6 +784,8 @@ static int alloc_table(tlag_engine* e, unsigned log2) {
   return TLAG_OK;
 }
 
+static int sync_store(tlag_engine* e, uint64_t n_states);
+
 static int grow_table_if_needed(tlag_engine* e, uint64_t expected_states) {
   const uint64_t slots = 1ULL << e->table_log2;
   if (expected_states * (e->tight ? 1 : 2) <= slots) return TLAG_OK;
@@ -791,6 +796,8 @@ static int grow_table_if_needed(tlag_engine* e, uint64_t expected_states) {
   int r = alloc_table(e, log2);
   if (r) return r;
   const uint64_t n = hc.n_states;
+  r = sync_store(e, n);            // the rehash reads every row from the store
+  if (r) return r;
   if (n) {
     k_rehash<<<(unsigned)((n + 255) / 256), 256, 0, e->stream>>>(e->p, n);
     e->launches++;
@@ -813,6 +820,11 @@ static int grow_store_if_needed(tlag_engine* e, uint64_t need) {
   cudaMemGetInfo(&freeb, &totalb);
   const uint64_t per = (uint64_t)e->m.words_per_state * 4 + 8;
   if (ncap * per > freeb * 9 / 10) {
+    // the clustering buffers are re-allocated by the next level that needs them: the store comes first (an open level
+    // keeps its discovery buffer, which holds its rows)
+    if (!e->disc_open) { dfree(e, e->d_disc); e->d_disc = nullptr; e->disc_bytes = 0; }
+    dfree(e, e->d_sort); e->d_sort = nullptr; e->sort_bytes = 0;
+    dfree(e, e->d_rset); e->d_rset = nullptr; e->rset_bytes = 0;
     trim_pool(e);
     cudaMemGetInfo(&freeb, &totalb);
   }
@@ -826,7 +838,7 @@ static int grow_store_if_needed(tlag_engine* e, uint64_t need) {
   CK(dmalloc(e, &nm, ncap * 4));
   Counters hc;
   CK(read_counters(e, &hc));
-  const uint64_t n = hc.n_states;
+  const uint64_t n = e->disc_open ? e->hi : hc.n_states;   // an open level's rows are in its discovery buffer
   CK(cudaMemcpyAsync(ns, e->d_states, n * (uint64_t)e->m.words_per_state * 4, cudaMemcpyDeviceToDevice, e->stream));
   CK(cudaMemcpyAsync(np, e->d_parent, n * 4, cudaMemcpyDeviceToDevice, e->stream));
   CK(cudaMemcpyAsync(nm, e->d_meta, n * 4, cudaMemcpyDeviceToDevice, e->stream));
@@ -834,7 +846,8 @@ static int grow_store_if_needed(tlag_engine* e, uint64_t need) {
   dfree(e, e->d_states); dfree(e, e->d_parent); dfree(e, e->d_meta);
   e->d_states = ns; e->d_parent = np; e->d_meta = nm;
   e->cap_states = ncap;
-  e->p.states = ns; e->p.parent = np; e->p.meta = nm; e->p.cap_states = ncap;
+  e->p.states = ns; e->p.parent = np; e->p.meta = nm;
+  if (!e->disc_open) point_appends(e);                   // an open level keeps appending to its buffer (open_level)
   return TLAG_OK;
 }
 
@@ -859,10 +872,32 @@ static bool ensure_cluster_buf(tlag_engine* e, void** buf, uint64_t* cap, uint64
   return true;
 }
 
+// Records [first, first + count) of the open level's discovery buffer into store rows [first, first + count): row
+// first + i gets record idx[i], or without idx record i (discovery order).
+static int gather_rows(tlag_engine* e, uint64_t first, uint64_t count, const uint32_t* idx) {
+  if (count == 0) return TLAG_OK;
+  const uint64_t W = e->m.words_per_state;
+  const uint32_t* rec = (const uint32_t*)e->d_disc + (first - e->hi) * (W + 2);
+  k_cluster_gather<<<(unsigned)((count + 255) / 256), 256, 0, e->stream>>>(rec, idx, count, (int)W, e->d_states + first * W,
+                                                                           e->d_parent + first, e->d_meta + first);
+  e->launches++;
+  CK(cudaGetLastError());
+  return TLAG_OK;
+}
+
+// Puts the open level's `count` discovered records into store rows [first, first + count): stably sorted by key, or in
+// discovery order when the level is not clustered (under 8192 states, TLAG_NO_SORT, a single key, or no device memory
+// for the pass: the order is an optimisation).
 static int cluster_slice(tlag_engine* e, uint64_t first, uint64_t count) {
   static const bool off = getenv("TLAG_NO_SORT") != nullptr;
-  if (off || count < 8192 || count > 0xFFFFFFFFull || (e->m.flags & TLAG_F_EXACT)) return TLAG_OK;   // exact: FIFO order is the point
+  // TLAG_CLUSTER_CHUNK_ORDER=1 keeps every key group contiguous and in ascending key order but changes the order inside
+  // it: the level's records enter the stable sort in chunks of 32 (one warp's), the chunks of each window of 64 in
+  // reverse -- the kind of order a counting sort gives whose groups are filled by per-warp cursor atomics.  Not a tuning
+  // knob: it measures what the order within a key costs the next waves (DESIGN.md section 4c).
+  static const bool chunk_order = getenv("TLAG_CLUSTER_CHUNK_ORDER") && atoi(getenv("TLAG_CLUSTER_CHUNK_ORDER")) != 0;
+  if (off || count < 8192 || count > 0xFFFFFFFFull) return gather_rows(e, first, count, nullptr);
   const uint64_t W = e->m.words_per_state;
+  const uint32_t* rec = (const uint32_t*)e->d_disc + (first - e->hi) * (W + 2);
   const uint64_t cpad = (count + 63) & ~63ull;
   size_t sort_tmp = 0, list_tmp = 0;
   {
@@ -872,36 +907,27 @@ static int cluster_slice(tlag_engine* e, uint64_t first, uint64_t count) {
     cub::DeviceRadixSort::SortKeys(nullptr, list_tmp, k64, (unsigned long long)count);   // the distinct keys: <= count
   }
   const size_t cub_bytes = sort_tmp > list_tmp ? sort_tmp : list_tmp;
-  // one scratch allocation: keys | A = (rank, idx) | B = (rank, idx) | records | cub temp.  The distinct keys are listed
-  // and sorted in A and B (as 64-bit words) before the states' ranks are written there.
-  const uint64_t rec_bytes = ((count * (W + 2) * 4) + 255) & ~255ull;
-  if (!ensure_cluster_buf(e, &e->d_sort, &e->sort_bytes, cpad * 8 * 3 + rec_bytes + cub_bytes, true)) return TLAG_OK;
+  // one scratch allocation: A = (slot, then rank | idx) | B = (rank | idx) | cub temp
+  if (!ensure_cluster_buf(e, &e->d_sort, &e->sort_bytes, cpad * 8 * 2 + cub_bytes, true)) return gather_rows(e, first, count, nullptr);
   uint8_t* b = (uint8_t*)e->d_sort;
-  unsigned long long* keys = (unsigned long long*)b; b += cpad * 8;
-  uint8_t* A = b; b += cpad * 8;
-  uint8_t* B = b; b += cpad * 8;
-  uint32_t* rec = (uint32_t*)b; b += rec_bytes;
-  void* cub_tmp = b;
-  uint32_t* st = e->d_states + first * W;
+  uint32_t* rank_a = (uint32_t*)b; uint32_t* idx_a = rank_a + cpad;
+  uint32_t* rank_b = idx_a + cpad; uint32_t* idx_b = rank_b + cpad;
+  void* cub_tmp = b + cpad * 16;
   const unsigned blocks = (unsigned)((count + 255) / 256);
-  k_cluster_pack<<<blocks, 256, 0, e->stream>>>(st, e->d_parent + first, e->d_meta + first, count, (int)W, rec, keys);
-  CK(cudaGetLastError());
-  e->launches++;
 
-  // the level's distinct keys; a set past half full is grown 4x and filled again
+  // the level's distinct keys and each record's slot; a set past half full is grown 4x and filled again
   unsigned log2 = e->rset_log2;
   RankSetCtl hc;
-  unsigned long long *table = nullptr;
-  uint32_t* rank = nullptr;
   for (;;) {
     const uint64_t slots = 1ull << log2;
-    if (!ensure_cluster_buf(e, &e->d_rset, &e->rset_bytes, 256 + slots * 12, false)) return TLAG_OK;
+    // [RankSetCtl | slots keys | slots + 2 ranks | two lists of slots / 2 keys]: a set that is not full holds <= slots / 2
+    if (!ensure_cluster_buf(e, &e->d_rset, &e->rset_bytes, 256 + slots * 8 + (slots + 2) * 4 + slots * 8, false))
+      return gather_rows(e, first, count, nullptr);
     RankSetCtl* ctl = (RankSetCtl*)e->d_rset;
-    table = (unsigned long long*)((uint8_t*)e->d_rset + 256);
-    rank = (uint32_t*)(table + slots);
+    unsigned long long* table = (unsigned long long*)((uint8_t*)e->d_rset + 256);
     CK(cudaMemsetAsync(ctl, 0, sizeof(RankSetCtl), e->stream));
     CK(cudaMemsetAsync(table, 0xFF, slots * 8, e->stream));
-    k_rset_insert<<<blocks, 256, 0, e->stream>>>(keys, count, table, slots - 1, ctl);
+    k_rset_insert<<<blocks, 256, 0, e->stream>>>(rec, count, (int)W, table, slots - 1, ctl, rank_a);
     CK(cudaGetLastError());
     e->launches++;
     CK(cudaMemcpyAsync(&hc, ctl, sizeof(hc), cudaMemcpyDeviceToHost, e->stream));
@@ -911,36 +937,99 @@ static int cluster_slice(tlag_engine* e, uint64_t first, uint64_t count) {
   }
   if (!e->rset_fixed) e->rset_log2 = log2;
   const uint64_t distinct = (uint64_t)hc.n + hc.has_max;
-  if (distinct <= 1) return TLAG_OK;                  // one key: the stable order is discovery order, already in place
+  if (distinct <= 1) return gather_rows(e, first, count, nullptr);   // one key: the stable order is discovery order
   const uint64_t slots = 1ull << log2;
   RankSetCtl* ctl = (RankSetCtl*)e->d_rset;
+  unsigned long long* table = (unsigned long long*)((uint8_t*)e->d_rset + 256);
+  uint32_t* rank = (uint32_t*)(table + slots);        // per slot, and one for the TLAG_RSET_EMPTY key
 
   // rank of each distinct key = its position in sorted order (a key equal to the empty marker is the largest: rank n)
-  k_rset_list<<<(unsigned)((slots + 255) / 256), 256, 0, e->stream>>>(table, slots, (unsigned long long*)A, ctl);
+  unsigned long long* list_a = (unsigned long long*)(rank + slots + 2);
+  unsigned long long* list_b = list_a + slots / 2;
+  k_rset_list<<<(unsigned)((slots + 255) / 256), 256, 0, e->stream>>>(table, slots, list_a, ctl);
   CK(cudaGetLastError());
-  cub::DoubleBuffer<unsigned long long> dk((unsigned long long*)A, (unsigned long long*)B);
+  cub::DoubleBuffer<unsigned long long> dk(list_a, list_b);
   size_t tb = cub_bytes;
   if (cub::DeviceRadixSort::SortKeys(cub_tmp, tb, dk, (unsigned long long)hc.n, 0, 64, e->stream) != cudaSuccess) {
     e->err = "cub sort failed"; return TLAG_ECUDA;
   }
-  k_rset_rank<<<(hc.n + 255) / 256, 256, 0, e->stream>>>(dk.Current(), hc.n, table, slots - 1, rank);
+  k_rset_rank<<<(hc.n + 1 + 255) / 256, 256, 0, e->stream>>>(dk.Current(), hc.n, table, slots - 1, rank);
   CK(cudaGetLastError());
 
-  // stable sort of (rank, discovery index) over the rank's bits, then one gather back into the store
-  uint32_t* rank_a = (uint32_t*)A; uint32_t* idx_a = rank_a + cpad;
-  uint32_t* rank_b = (uint32_t*)B; uint32_t* idx_b = rank_b + cpad;
-  k_rank_states<<<blocks, 256, 0, e->stream>>>(keys, count, table, slots - 1, rank, hc.n, rank_a, idx_a);
+  // stable sort of (rank, discovery index) over the rank's bits, then one gather from the buffer into the store
+  // (in place over the slots; a reordered input is written to B, whose entries the sort starts from)
+  uint32_t *rank_in = chunk_order ? rank_b : rank_a, *idx_in = chunk_order ? idx_b : idx_a;
+  k_rank_states<<<blocks, 256, 0, e->stream>>>(rank_a, count, rank, rank_in, idx_in, chunk_order ? 1 : 0);
   CK(cudaGetLastError());
   const int end_bit = 32 - __builtin_clz((unsigned)(distinct - 1));
-  cub::DoubleBuffer<uint32_t> rk(rank_a, rank_b), ix(idx_a, idx_b);
+  cub::DoubleBuffer<uint32_t> rk(rank_in, chunk_order ? rank_a : rank_b), ix(idx_in, chunk_order ? idx_a : idx_b);
   tb = cub_bytes;
   if (cub::DeviceRadixSort::SortPairs(cub_tmp, tb, rk, ix, (unsigned long long)count, 0, end_bit, e->stream) != cudaSuccess) {
     e->err = "cub sort failed"; return TLAG_ECUDA;
   }
-  k_cluster_gather<<<blocks, 256, 0, e->stream>>>(rec, ix.Current(), count, (int)W, st, e->d_parent + first,
-                                                  e->d_meta + first);
-  CK(cudaGetLastError());
   e->launches += 4;
+  return gather_rows(e, first, count, ix.Current());
+}
+
+// Rows the open level has discovered so far, copied into the store in discovery order, for a call that reads the store
+// in the middle of a level.  The buffer keeps them: the level is still clustered when it ends.
+static int sync_store(tlag_engine* e, uint64_t n_states) {
+  if (!e->disc_open) return TLAG_OK;
+  const uint64_t end = n_states < e->p.cap_states ? n_states : e->p.cap_states;
+  if (end <= e->hi) return TLAG_OK;
+  int r = gather_rows(e, e->hi, end - e->hi, nullptr);
+  if (r) return r;
+  CK(cudaStreamSynchronize(e->stream));
+  return TLAG_OK;
+}
+
+// The level appends to the store itself again: its discovery buffer's rows are in the store, or discarded.
+static void end_appends(tlag_engine* e) {
+  e->disc_open = false;
+  point_appends(e);
+}
+
+// Opens the level being discovered for appends to the discovery buffer: rows [hi, hi + rows) of it, at most up to the
+// store's capacity.  A row past that is counted in n_states, not written, and reported as a store overflow.  A level that
+// is already open keeps the rows it has put there, and its room never shrinks.  Without device memory for the buffer the
+// level appends to the store itself and is not clustered.  TLAG_F_EXACT always does: its single worker dequeues the rows
+// it appends, in the same launch.
+static int open_level(tlag_engine* e, uint64_t rows) {
+  if (e->m.flags & TLAG_F_EXACT) return TLAG_OK;
+  const uint64_t room = e->cap_states - e->hi;
+  if (rows > room) rows = room;
+  if (e->disc_open && e->p.cap_states >= e->hi + rows) return TLAG_OK;
+  const uint64_t rb = (e->m.words_per_state + 2) * 4;
+  if (rows * rb > e->disc_bytes) {
+    uint64_t used = 0;
+    if (e->disc_open) {
+      Counters hc;
+      CK(read_counters(e, &hc));
+      used = (hc.n_states < e->p.cap_states ? hc.n_states : e->p.cap_states) - e->hi;
+    }
+    // levels grow: twice the rows asked for while the store has room for them, so that the next levels fit too (only
+    // from memory that is free: the pool is not trimmed for it)
+    uint64_t want = (rows * 2 < room ? rows * 2 : room) * rb;
+    void* nb = nullptr;
+    if (want > rows * rb && dmalloc(e, &nb, want, false) != cudaSuccess) { cudaGetLastError(); nb = nullptr; }
+    if (!nb) {
+      want = rows * rb;
+      if (dmalloc(e, &nb, want) != cudaSuccess) {
+        cudaGetLastError();
+        int r = used ? gather_rows(e, e->hi, used, nullptr) : TLAG_OK;
+        if (r) return r;
+        dfree(e, e->d_disc); e->d_disc = nullptr; e->disc_bytes = 0;
+        end_appends(e);
+        return TLAG_OK;
+      }
+    }
+    if (used) CK(cudaMemcpyAsync(nb, e->d_disc, used * rb, cudaMemcpyDeviceToDevice, e->stream));
+    dfree(e, e->d_disc);
+    e->d_disc = nb; e->disc_bytes = want;
+  }
+  e->disc_open = true;
+  point_appends(e);
+  e->p.cap_states = e->hi + rows;
   return TLAG_OK;
 }
 
@@ -1055,6 +1144,7 @@ extern "C" int tlag_create(const tlag_model* m, tlag_engine** out) {
   e->p.entry_inv = m->entry_inv; e->p.entry_next = m->entry_next;
   e->p.n_off = 0; e->p.p_off = m->unpacked_words; e->p.W = (int)m->words_per_state;
   e->p.states = e->d_states; e->p.parent = e->d_parent; e->p.meta = e->d_meta; e->p.cap_states = cap;
+  point_appends(e);
   e->p.ctr = e->d_ctr; e->p.flags = m->flags; e->p.n_inv = (int)m->n_invariants;
   e->p.n_ranks = 1; e->p.rank = 0; e->p.owner_words = 2;
   // Sliced build: a successor whose packed words equal its parent's is counted (generated, has-a-successor) and dropped
@@ -1094,7 +1184,7 @@ extern "C" void tlag_destroy(tlag_engine* e) {
   cudaFree(e->d_code); cudaFree(e->d_cpool); cudaFree(e->d_layout); cudaFree(e->d_ctr); cudaFree(e->d_dig);
   if (e->stream) {
     dfree(e, e->d_states); dfree(e, e->d_parent); dfree(e, e->d_meta); dfree(e, e->d_table);
-    dfree(e, e->d_scratch); dfree(e, e->d_flags); dfree(e, e->d_sort); dfree(e, e->d_rset); dfree(e, e->d_sent); dfree(e, e->d_succ);
+    dfree(e, e->d_scratch); dfree(e, e->d_flags); dfree(e, e->d_disc); dfree(e, e->d_sort); dfree(e, e->d_rset); dfree(e, e->d_sent); dfree(e, e->d_succ);
     cudaStreamSynchronize(e->stream);
   }
   if (e->p2p_slot >= 0) {                              // exchange buffers and peer mappings are parked, not released
@@ -1211,6 +1301,7 @@ extern "C" int tlag_seed(tlag_engine* e, const uint32_t* states, uint64_t n) {
 // Forget everything discovered and start again from the retained initial states (bench loops).
 extern "C" int tlag_restart(tlag_engine* e) {
   if (!e) return TLAG_EINVAL;
+  end_appends(e);
   CK(reset_counters(e, 0));
   CK(cudaMemsetAsync(e->d_table, 0, (1ULL << e->table_log2) * 8, e->stream));
   if (e->d_sent) CK(cudaMemsetAsync(e->d_sent, 0, (e->p.sent_mask + 1) * 8, e->stream));
@@ -1292,14 +1383,17 @@ static int account_wave(tlag_engine* e, const Counters& hc, bool keep_going, uin
   return TLAG_OK;
 }
 
-// head-room for the next level: twice the observed discovered/expanded ratio, at least 4x
+// head-room for the next level: in the store twice the observed discovered/expanded ratio, at least 4x; in the discovery
+// buffer the ratio plus a quarter (a level that outgrows it is rolled back and redone, tlag_step)
 static void note_growth(tlag_engine* e, uint64_t expanded, uint64_t discovered) {
   const double ratio = (double)discovered / (double)(expanded ? expanded : 1);
   e->growth_hint = ratio * 2.0 > 4.0 ? ratio * 2.0 : 4.0;
+  e->disc_hint = ratio * 1.25;
 }
 
-// End of a level whose store now holds n_states states: the slice it appended (if any) sets the depth and, with
-// cluster, is put in clustering order (device time in out->cluster_ms); then it becomes the frontier.
+// End of a level whose store now holds n_states states: the slice it appended (if any) sets the depth and goes from the
+// discovery buffer into the store, with cluster in clustering order, else in discovery order (device time in
+// out->cluster_ms); then it becomes the frontier.
 static int close_level(tlag_engine* e, uint64_t n_states, bool cluster, tlag_wave_stats* out) {
   if (out) {
     out->level = e->level; out->discovered = n_states - e->hi; out->distinct_total = n_states;
@@ -1307,13 +1401,17 @@ static int close_level(tlag_engine* e, uint64_t n_states, bool cluster, tlag_wav
   }
   if (n_states > e->hi) {
     e->depth = e->level + 1;
-    if (cluster) {
+    if (e->disc_open) {
+      const uint64_t n = (n_states < e->p.cap_states ? n_states : e->p.cap_states) - e->hi;
       float ms = 0;
-      int r = timed(e, &ms, nullptr, [&] { return cluster_slice(e, e->hi, n_states - e->hi); });
+      int r = timed(e, &ms, nullptr, [&] {
+        return cluster ? cluster_slice(e, e->hi, n) : gather_rows(e, e->hi, n, nullptr);
+      });
       if (r) return r;
       if (out) out->cluster_ms = ms;
     }
   }
+  end_appends(e);
   e->lo = e->hi; e->hi = n_states; e->level += 1;
   return TLAG_OK;
 }
@@ -1322,6 +1420,7 @@ static int close_level(tlag_engine* e, uint64_t n_states, bool cluster, tlag_wav
 // seen-set is rebuilt from the store (it holds fingerprints of the dropped states) and every other counter is reset --
 // the level is then expanded again from scratch with more room.
 static int rollback_wave(tlag_engine* e, uint64_t hi, uint64_t want_states) {
+  end_appends(e);                  // the discovery buffer's rows are dropped with them
   CK(reset_counters(e, hi));
   int r = grow_store_if_needed(e, e->tight ? want_states : want_states + 4096);
   if (r) return r;
@@ -1353,10 +1452,15 @@ extern "C" int tlag_step(tlag_engine* e, tlag_wave_stats* out) {
                         e->tight ? hi + (hi - lo)
                                  : hi + (uint64_t)((double)(hi - lo) * (e->growth_hint > 4.0 ? e->growth_hint * 0.5 : 2.0)));
   if (r) return r;
+  // the level's new rows go to the discovery buffer, sized from the previous level's growth (a rerun: from its count);
+  // TLAG_TIGHT_HEADROOM sizes the store alone, and the buffer takes all of its room
+  uint64_t rows = e->tight ? e->cap_states - hi : (uint64_t)((double)(hi - lo) * e->disc_hint) + 4096;
   Counters hc;
   float ms = 0;
   int attempt = 0;
   for (;; ++attempt) {
+    r = open_level(e, rows);
+    if (r) return r;
     CK(cudaMemsetAsync(&e->d_ctr->work, 0, 8, e->stream));
     float ms1 = 0;
     r = timed(e, &ms1, &hc, [&] { CK(launch_wave<0>(e, lo, hi)); return TLAG_OK; });
@@ -1373,6 +1477,7 @@ extern "C" int tlag_step(tlag_engine* e, tlag_wave_stats* out) {
     r = rollback_wave(e, hi, want);
     if (r) return r;
     if (e->cap_states < need + (e->tight ? 0 : 1024)) { e->err = "state store overflow: not enough device memory for this level"; return TLAG_ENOMEM; }
+    rows = e->tight ? e->cap_states - hi : want - hi;
   }
   e->dev_seconds += ms * 1e-3;
   r = account_wave(e, hc, (e->m.flags & TLAG_F_KEEP_GOING) != 0, hi - lo, ms, out);
@@ -1410,6 +1515,8 @@ extern "C" int tlag_read_states(tlag_engine* e, uint64_t first, uint64_t n, uint
   Counters hc;
   CK(read_counters(e, &hc));
   if (first + n > hc.n_states) { e->err = "tlag_read_states: range beyond the state store"; return TLAG_EINVAL; }
+  int r = sync_store(e, hc.n_states);
+  if (r) return r;
   const uint64_t W = e->m.words_per_state;
   CK(cudaMemcpy(states_out, e->d_states + first * W, n * W * 4, cudaMemcpyDeviceToHost));
   return TLAG_OK;
@@ -1419,6 +1526,8 @@ extern "C" int tlag_digest(tlag_engine* e, uint64_t* xor_out, uint64_t* sum_out)
   if (!e || !xor_out || !sum_out) return TLAG_EINVAL;
   Counters hc;
   CK(read_counters(e, &hc));
+  int r = sync_store(e, hc.n_states);
+  if (r) return r;
   if (!e->d_dig) CK(cudaMalloc(&e->d_dig, 16));
   unsigned long long* d2 = e->d_dig;
   CK(cudaMemsetAsync(d2, 0, 16, e->stream));
@@ -1451,6 +1560,8 @@ extern "C" int tlag_trace(tlag_engine* e, uint64_t state_idx, uint32_t* states_o
   Counters hc;
   CK(read_counters(e, &hc));
   if (state_idx >= hc.n_states) { e->err = "tlag_trace: no such state"; return TLAG_EINVAL; }
+  int r0 = sync_store(e, hc.n_states);
+  if (r0) return r0;
   const uint64_t W = e->m.words_per_state;
   std::vector<uint32_t> words;   // the chain's states from state_idx back, while they fit the caller's buffer
   std::vector<int32_t> acts;
@@ -1481,7 +1592,8 @@ extern "C" int tlag_read_link(tlag_engine* e, uint64_t idx, uint32_t* state_out,
   Counters hc;
   CK(read_counters(e, &hc));
   if (idx >= hc.n_states) { e->err = "tlag_read_link: no such state"; return TLAG_EINVAL; }
-  return read_link(e, idx, state_out, parent_out, meta_out);
+  int r = sync_store(e, hc.n_states);
+  return r ? r : read_link(e, idx, state_out, parent_out, meta_out);
 }
 
 // ---- multi-GPU building blocks -----------------------------------------------------
@@ -1524,6 +1636,10 @@ extern "C" int tlag_expand_route(tlag_engine* e, uint32_t n_ranks, uint64_t firs
   }
   int r = ensure_sent_cache(e);
   if (r) return r;
+  // successors this rank owns itself are appended here (sliced build), room for them as tlag_p2p_level reserves it;
+  // an overflow is reported by tlag_insert_records
+  r = open_level(e, (uint64_t)((double)(e->hi - e->lo) * e->growth_hint) + 4096);
+  if (r) return r;
   e->p.send = (uint32_t*)(uintptr_t)d_send;
   e->p.region_cap = cap_records / n_ranks;
   CK(cudaMemsetAsync(&e->d_ctr->work, 0, 8, e->stream));
@@ -1554,6 +1670,8 @@ extern "C" int tlag_insert_records(tlag_engine* e, uint64_t d_recv, uint64_t n_r
   CK(read_counters(e, &hc));
   const uint64_t before = hc.n_states;
   int r = reserve_level(e, before + n_records + 1024, before + n_records);
+  if (r) return r;
+  r = open_level(e, before + n_records + 1024 - e->hi);   // the reservation: a store overflow fails this call
   if (r) return r;
   if (n_records) {
     float ms = 0;
@@ -1663,6 +1781,8 @@ extern "C" int tlag_p2p_level(tlag_engine* e, uint64_t n_chunks, uint64_t chunk_
   const uint64_t before = hc.n_states;
   e->p2p_level_start = before; e->p2p_level_generated = 0;
   int r = reserve_level(e, before + expect, before + expect);
+  if (r) return r;
+  r = open_level(e, before + expect - e->hi);    // the level's reservation: a store overflow fails the level
   if (r) return r;
   e->p.n_ranks = (int)n_ranks; e->p.rank = e->q.rank;
   r = ensure_sent_cache(e);

@@ -3,10 +3,12 @@ with tlag_step, after `--warmup` untimed runs of the same job on the same engine
 states expanded, successors generated, states discovered, the wave kernels' time (CUDA events around the level's
 invariant, Next and deadlock kernels) and the time of the frontier clustering pass that reorders the level's new states
 (`cluster_ms`, with the bytes a reorder cannot avoid -- every record of W words + parent + meta read once and written
-once -- and the rate that gives), the job's wall time, whether the counts and the digest match the oracle's record,
-the TLAG_SL_* switches in effect, and the GPU's name, power limit and maximum SM clock.
+once -- and the rate that gives), the level's reruns after a store overflow (`retries`), the job's wall time, whether
+the counts and the digest match the oracle's record, the TLAG_SL_* switches in effect, and the GPU's name, power limit
+and maximum SM clock.  With --kernels the timed job runs under torch.profiler instead, and the line gets the device
+time of every kernel over the job (`kernels`, ms by name); its wall time then includes the tracing.
 
-    python tools/wave_profile.py [MCPaxos3_b4] [--warmup 1] [--max-levels L]
+    python tools/wave_profile.py [MCPaxos3_b4] [--warmup 1] [--max-levels L] [--kernels]
 """
 import argparse
 import json
@@ -51,6 +53,7 @@ def main():
     ap.add_argument("fixture", nargs="?", default="MCPaxos3_b4")
     ap.add_argument("--warmup", type=int, default=1)
     ap.add_argument("--max-levels", type=int, default=0, help="stop after this many levels (default: the fixture's bound)")
+    ap.add_argument("--kernels", action="store_true", help="per-kernel device times of the timed job (torch.profiler)")
     args = ap.parse_args()
     if args.max_levels < 0:
         ap.error("--max-levels must be at least 1 (0: the fixture's bound)")
@@ -73,9 +76,14 @@ def main():
             ws = e.step()
             lv += 1
             if ws["expanded"]:
-                reorder = 2 * (cm.W + 2) * 4 * ws["discovered"] if ws["cluster_ms"] > 0 else 0
+                # levels the pass sorts (an unclustered level is copied in discovery order, or appended to the store
+                # when no discovery buffer fitted: not counted as a reorder)
+                sorted_ = (ws["cluster_ms"] > 0 and ws["discovered"] >= 8192 and ws["verdict"] == V_RUNNING
+                           and not os.environ.get("TLAG_NO_SORT"))
+                reorder = 2 * (cm.W + 2) * 4 * ws["discovered"] if sorted_ else 0
                 levels.append({k: ws[k] for k in ("level", "expanded", "generated", "discovered")}
-                              | {"kernel_ms": round(ws["kernel_ms"], 3), "cluster_ms": round(ws["cluster_ms"], 3),
+                              | {"retries": ws["retries"],
+                                 "kernel_ms": round(ws["kernel_ms"], 3), "cluster_ms": round(ws["cluster_ms"], 3),
                                  "reorder_bytes": reorder,
                                  "reorder_gb_s": round(reorder / ws["cluster_ms"] * 1e-6, 1) if reorder else 0.0})
             if ws["verdict"] != V_RUNNING:
@@ -85,8 +93,22 @@ def main():
     for _ in range(max(0, args.warmup)):
         job(False)
         e.restart()
+    kernels = None
     t0 = time.perf_counter()
-    levels = job(True)
+    if args.kernels:
+        import torch
+        from torch.profiler import ProfilerActivity, profile
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            levels = job(True)
+            torch.cuda.synchronize()
+        kernels = {}
+        for a in prof.key_averages():     # device time per kernel / copy / memset name, microseconds -> ms
+            us = getattr(a, "self_device_time_total", None) or getattr(a, "self_cuda_time_total", 0)
+            if us > 0:
+                kernels[a.key[:120]] = kernels.get(a.key[:120], 0.0) + us * 1e-3
+        kernels = {k: round(v, 3) for k, v in sorted(kernels.items(), key=lambda kv: -kv[1])}
+    else:
+        levels = job(True)
     wall = time.perf_counter() - t0
     r = e.result()
     counts_ok = (r["generated"], r["distinct"], r["depth"]) == (o2["generated"], o2["distinct"], o2["depth"])
@@ -102,6 +124,7 @@ def main():
                       "other_s": round(wall - (kern + clus) * 1e-3, 4), "counts_match_oracle": counts_ok,
                       "digest_matches_oracle": digest_ok,
                       "switches": switches(),
+                      **({"kernels": kernels} if kernels is not None else {}),
                       "gpu": gpu_info(os.environ.get("CUDA_VISIBLE_DEVICES", "0").split(",")[0] or "0"),
                       "levels": levels}))
 
