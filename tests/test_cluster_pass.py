@@ -5,17 +5,14 @@ keys and one gather back into the store.  On the sliced native kernels, for a sc
 - every clustered level reads back ordered by (w[W-1], w[W-2]), and holds exactly the oracle's states of that level;
 - sampled parent links point into the previous level;
 - counts, per-level sizes and digests match the oracle with the rank set at its default size, with a rank set of
-  4 slots (TLAG_RSET_SLOTS, read when the engine is created: it fills up and grows on every clustered level), and
-  with the pass switched off (TLAG_NO_SORT=1, read once per process: a child process)."""
-import json
+  4 slots (TLAG_RSET_SLOTS: it fills up and grows on every clustered level), and with the pass switched off
+  (TLAG_NO_SORT=1).  Both are read when the engine is created."""
 import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
 
-from conftest import GOLDEN, ROOT
+from conftest import GOLDEN
 from tla_rust_b200.compiled import load_compiled
 
 # MCPaxos3_b3 is scalar form (W = 8, 8.2 M states), MCraft_t4l3 array form (W = 62, 11.3 M states); the level-by-level
@@ -101,18 +98,12 @@ def test_a_tiny_rank_set_grows_and_changes_nothing(monkeypatch, name):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("name", NAMES)
-def test_without_clustering_the_counts_and_digests_are_the_same(name):
+def test_without_clustering_the_counts_and_digests_are_the_same(monkeypatch, name):
+    monkeypatch.setenv("TLAG_NO_SORT", "1")
+    monkeypatch.delenv("TLAG_RSET_SLOTS", raising=False)
     want_levels, want_counts, want_digest = _expect(name)
-    code = (f"import json, sys; sys.path.insert(0, {ROOT!r}); sys.path.insert(0, {os.path.join(ROOT, 'tests')!r})\n"
-            f"import test_cluster_pass as t\n"
-            f"e, levels, r = t._run({name!r})\n"
-            f"print(json.dumps([levels, [r['generated'], r['distinct'], r['depth']], list(e.digest())]))\n"
-            f"e.close()\n")
-    env = dict(os.environ, TLAG_NO_SORT="1")
-    env.pop("TLAG_RSET_SLOTS", None)
-    out = subprocess.run([sys.executable, "-c", code], env=env, capture_output=True, text=True, timeout=900)
-    assert out.returncode == 0, out.stderr[-3000:]
-    levels, counts, digest = json.loads(out.stdout.strip().splitlines()[-1])
+    e, levels, r = _run(name)
     assert levels == want_levels
-    assert tuple(counts) == want_counts
-    assert tuple(digest) == want_digest
+    assert (r["generated"], r["distinct"], r["depth"]) == want_counts
+    assert e.digest() == want_digest
+    e.close()

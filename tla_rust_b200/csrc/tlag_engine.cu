@@ -30,13 +30,11 @@
 #undef TLAG_VM_EXEC_FN
 #undef TLAG_VM_EXT
 
-// Resident CTAs per SM the interpreter wave kernel is compiled for (register cap = 65536 / (512 x this)).
-#define TLAG_WAVE_OCC(FRAME, SMEM) ((FRAME) <= 256 ? 4 : ((FRAME) <= 512 ? 2 : ((SMEM) ? 1 : TLAG_BIG_OCC)))
+// Resident CTAs per SM the interpreter wave kernel is compiled for (register cap = 65536 / (512 x this)).  Big frames
+// (> 512 words) with the image in global memory get 4: they are latency-bound on local memory.
+#define TLAG_WAVE_OCC(FRAME, SMEM) ((FRAME) <= 256 ? 4 : ((FRAME) <= 512 ? 2 : ((SMEM) ? 1 : 4)))
 
 #define TLAG_MAXW 128
-#ifndef TLAG_BIG_OCC
-#define TLAG_BIG_OCC 4   /* resident CTAs per SM for the big-frame (> 512 words) wave kernels: latency-bound on local memory */
-#endif
 #define TLAG_BLOCK 512
 #define TLAG_MAX_STEPS (1u << 26)
 
@@ -73,7 +71,8 @@ struct tlag_engine {
   int frame_class = 0;
   bool uses_ext = false;            // the image contains LEXLT / SFIND / SINS / EMITD (full interpreter needed)
   bool restarting = false;
-  bool tight = false;               // TLAG_TIGHT_HEADROOM (test hook): store and table sized for no growth, see tlag_create
+  bool tight = false;               // TLAG_TIGHT_HEADROOM (test hook): store and table sized for no growth, see read_env_hooks
+  bool no_sort = false;             // TLAG_NO_SORT (test hook): levels go to the store in discovery order, see cluster_slice
   double growth_hint = 4.0;
   double disc_hint = 4.0;           // discovery buffer rows per state expanded, for the next level (note_growth)
   // discovery buffer: the open level's new rows (DevParams::disc), put into the store by close_level
@@ -531,21 +530,15 @@ __global__ void k_rset_rank(const unsigned long long* __restrict__ sorted, unsig
   else if (i == n) rank[mask + 1] = n;
 }
 
-// Entry i of the sort: the rank of record j and j itself, j = i (rank_out may be `slot`: each thread reads its own
-// entry before it writes it).  chunk_order: in every full window of 64 chunks of 32 records the chunks enter in reverse
-// order (TLAG_CLUSTER_CHUNK_ORDER, cluster_slice).
+// Entry i of the sort: the rank of record i and i itself (rank_out may be `slot`: each thread reads its own entry
+// before it writes it).
 __global__ void k_rank_states(const uint32_t* slot, unsigned long long n, const uint32_t* __restrict__ rank,
-                              uint32_t* rank_out, uint32_t* __restrict__ idx, int chunk_order) {
+                              uint32_t* rank_out, uint32_t* __restrict__ idx) {
   const unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  unsigned long long j = i;
-  if (chunk_order) {
-    const unsigned long long c = i >> 5, w = c & ~63ull;
-    if ((w + 64) * 32 <= n) j = ((w | (63 - (c & 63))) << 5) | (i & 31);
-  }
-  const uint32_t r = __ldg(rank + slot[j]);
+  const uint32_t r = __ldg(rank + slot[i]);
   rank_out[i] = r;
-  idx[i] = (uint32_t)j;
+  idx[i] = (uint32_t)i;
 }
 
 // Store row first + i <- record idx[i] of the discovery buffer (st, parent and meta point at row first; without idx,
@@ -623,8 +616,6 @@ static void trim_pool(tlag_engine* e) {
   cudaGetLastError();
 }
 static cudaError_t dmalloc(tlag_engine* e, void* pp, size_t bytes, bool trim = true) {
-  static const bool plain = getenv("TLAG_NO_POOL") != nullptr;
-  if (plain) return cudaMalloc((void**)pp, bytes);
   cudaError_t r = cudaMallocAsync((void**)pp, bytes, e->stream);
   if (r == cudaErrorMemoryAllocation && trim) {
     cudaGetLastError();
@@ -634,9 +625,7 @@ static cudaError_t dmalloc(tlag_engine* e, void* pp, size_t bytes, bool trim = t
   return r;
 }
 static void dfree(tlag_engine* e, void* p) {
-  static const bool plain = getenv("TLAG_NO_POOL") != nullptr;
-  if (!p) return;
-  if (plain) cudaFree(p); else cudaFreeAsync(p, e->stream);
+  if (p) cudaFreeAsync(p, e->stream);
 }
 
 // DevParams::app at the store, or with the level open at its discovery buffer (row hi = record 0).  The store's append
@@ -889,13 +878,7 @@ static int gather_rows(tlag_engine* e, uint64_t first, uint64_t count, const uin
 // discovery order when the level is not clustered (under 8192 states, TLAG_NO_SORT, a single key, or no device memory
 // for the pass: the order is an optimisation).
 static int cluster_slice(tlag_engine* e, uint64_t first, uint64_t count) {
-  static const bool off = getenv("TLAG_NO_SORT") != nullptr;
-  // TLAG_CLUSTER_CHUNK_ORDER=1 keeps every key group contiguous and in ascending key order but changes the order inside
-  // it: the level's records enter the stable sort in chunks of 32 (one warp's), the chunks of each window of 64 in
-  // reverse -- the kind of order a counting sort gives whose groups are filled by per-warp cursor atomics.  Not a tuning
-  // knob: it measures what the order within a key costs the next waves (DESIGN.md section 4c).
-  static const bool chunk_order = getenv("TLAG_CLUSTER_CHUNK_ORDER") && atoi(getenv("TLAG_CLUSTER_CHUNK_ORDER")) != 0;
-  if (off || count < 8192 || count > 0xFFFFFFFFull) return gather_rows(e, first, count, nullptr);
+  if (e->no_sort || count < 8192 || count > 0xFFFFFFFFull) return gather_rows(e, first, count, nullptr);
   const uint64_t W = e->m.words_per_state;
   const uint32_t* rec = (const uint32_t*)e->d_disc + (first - e->hi) * (W + 2);
   const uint64_t cpad = (count + 63) & ~63ull;
@@ -957,12 +940,11 @@ static int cluster_slice(tlag_engine* e, uint64_t first, uint64_t count) {
   CK(cudaGetLastError());
 
   // stable sort of (rank, discovery index) over the rank's bits, then one gather from the buffer into the store
-  // (in place over the slots; a reordered input is written to B, whose entries the sort starts from)
-  uint32_t *rank_in = chunk_order ? rank_b : rank_a, *idx_in = chunk_order ? idx_b : idx_a;
-  k_rank_states<<<blocks, 256, 0, e->stream>>>(rank_a, count, rank, rank_in, idx_in, chunk_order ? 1 : 0);
+  // (in place over the slots)
+  k_rank_states<<<blocks, 256, 0, e->stream>>>(rank_a, count, rank, rank_a, idx_a);
   CK(cudaGetLastError());
   const int end_bit = 32 - __builtin_clz((unsigned)(distinct - 1));
-  cub::DoubleBuffer<uint32_t> rk(rank_in, chunk_order ? rank_a : rank_b), ix(idx_in, chunk_order ? idx_a : idx_b);
+  cub::DoubleBuffer<uint32_t> rk(rank_a, rank_b), ix(idx_a, idx_b);
   tb = cub_bytes;
   if (cub::DeviceRadixSort::SortPairs(cub_tmp, tb, rk, ix, (unsigned long long)count, 0, end_bit, e->stream) != cudaSuccess) {
     e->err = "cub sort failed"; return TLAG_ECUDA;
@@ -1034,9 +1016,9 @@ static int open_level(tlag_engine* e, uint64_t rows) {
 }
 
 // Route mode with several ranks: the direct-mapped cache of the fingerprints this rank has routed (2^26 x 8 B = 512 MB).
-// It is only a filter: without memory for it, or with TLAG_NO_SENT_CACHE set, every successor is routed.
+// It is only a filter: without memory for it every successor is routed.
 static int ensure_sent_cache(tlag_engine* e) {
-  if (e->d_sent || e->p.n_ranks < 2 || getenv("TLAG_NO_SENT_CACHE") != nullptr) return TLAG_OK;
+  if (e->d_sent || e->p.n_ranks < 2) return TLAG_OK;
   const unsigned long long slots = 1ULL << 26;
   if (dmalloc(e, &e->d_sent, slots * 8) != cudaSuccess) { cudaGetLastError(); e->d_sent = nullptr; return TLAG_OK; }
   CK(cudaMemsetAsync(e->d_sent, 0, slots * 8, e->stream));
@@ -1053,6 +1035,34 @@ extern "C" const char* tlag_version(void) { return "tlag 0.1 (sm_90a)"; }
 extern "C" const char* tlag_last_error(const tlag_engine* e) { return e ? e->err.c_str() : "null engine"; }
 
 extern "C" uint64_t tlag_kernel_launches(const tlag_engine* e) { return e ? e->launches : 0; }
+
+// The engine's test hooks (DESIGN.md section 4d), read once per engine: each forces a path that a test must reach and
+// that the engine's own sizing would rarely or never take.  None is a tuning knob.  Called with e->p zeroed.
+static void read_env_hooks(tlag_engine* e) {
+  // 1: the store starts at 1024 rows, and the store and the seen-set are sized before each level for as many new states
+  // as the level expands, with no slack, and a rerun for exactly what the failed attempt counted: every level that grows
+  // overflows the store (or, with a small table_slots_log2, fills the table) and is rolled back and redone (rollback_wave)
+  const char* s_ = getenv("TLAG_TIGHT_HEADROOM");
+  e->tight = s_ && *s_ && atoi(s_) != 0;
+  // set (any value): no level is clustered, each goes to the store in discovery order (cluster_slice)
+  e->no_sort = getenv("TLAG_NO_SORT") != nullptr;
+  // sliced build: 0 probes self-loop successors like any other successor instead of dropping them at the emit site
+  s_ = getenv("TLAG_SL_SKIPSELF");
+  e->p.skip_self = (s_ && *s_) ? (atoi(s_) != 0) : 1;
+  // sliced build, scalar form: n caps the per-warp staging slots below the compiled number, so that the buffer fills up
+  // and the direct path runs (0: every successor is probed where it is produced; tlag_dev.cuh, TLAG_SL_STAGED)
+  s_ = getenv("TLAG_SL_STAGE");
+  e->p.stage = (s_ && *s_) ? (atoi(s_) > 0 ? atoi(s_) : 0) : INT_MAX;
+  // n starts the clustering pass's rank set at n slots (rounded up to a power of two) on every level, so that it fills
+  // up and grows
+  s_ = getenv("TLAG_RSET_SLOTS");
+  if (s_ && *s_) {
+    const long n = atol(s_);
+    e->rset_log2 = 1;
+    while (e->rset_log2 < 40 && (1L << e->rset_log2) < n) ++e->rset_log2;
+    e->rset_fixed = true;
+  }
+}
 
 extern "C" int tlag_create(const tlag_model* m, tlag_engine** out) {
   if (!m || !out) return TLAG_EINVAL;
@@ -1096,7 +1106,6 @@ extern "C" int tlag_create(const tlag_model* m, tlag_engine** out) {
   CK(cudaEventCreate(&e->ev1));
   e->frame_class = 7;
   for (int i = 0; i < 8; ++i) if ((int)m->frame_words <= kFrameClasses[i]) { e->frame_class = i; break; }
-  e->uses_ext = getenv("TLAG_VM_FULL") != nullptr;
   for (uint32_t i = 0; i < m->code_len && !e->uses_ext; ++i) {
     const uint32_t op = (uint32_t)(m->code[i] & 0xFF);
     if (op == OP_LEXLT || op == OP_SFIND || op == OP_SINS || op == OP_EMITD || op == OP_CALL || op == OP_RET) e->uses_ext = true;
@@ -1110,14 +1119,8 @@ extern "C" int tlag_create(const tlag_model* m, tlag_engine** out) {
   CK(cudaMemcpy(e->d_layout, m->layout, (size_t)m->n_slots * sizeof(tlag_slot), cudaMemcpyHostToDevice));
   CK(cudaMalloc(&e->d_ctr, sizeof(Counters)));
   CK(reset_counters(e, 0));
-  // TLAG_TIGHT_HEADROOM=1 starts the store at 1024 rows and sizes the store and the seen-set before each level for as many
-  // new states as the level expands, with no slack, and a rerun for exactly what the failed attempt counted: every level
-  // that grows then overflows the store (or, with a small table_slots_log2, fills the table) and is rolled back and
-  // redone (rollback_wave).  Tests use it to run that path; not a tuning knob.
-  {
-    const char* s_ = getenv("TLAG_TIGHT_HEADROOM");
-    e->tight = s_ && *s_ && atoi(s_) != 0;
-  }
+  memset(&e->p, 0, sizeof(e->p));
+  read_env_hooks(e);
   // state store
   uint64_t cap = m->max_states ? m->max_states : (1ULL << 20);
   if (cap < 1024) cap = 1024;
@@ -1128,18 +1131,12 @@ extern "C" int tlag_create(const tlag_model* m, tlag_engine** out) {
   CK(dmalloc(e, &e->d_states, cap * (uint64_t)m->words_per_state * 4));
   CK(dmalloc(e, &e->d_parent, cap * 4));
   CK(dmalloc(e, &e->d_meta, cap * 4));
-  memset(&e->p, 0, sizeof(e->p));
   e->p.code = e->d_code; e->p.code_len = m->code_len;
-  {
-    // bytecode image in shared memory when it fits; TLAG_CODE_SMEM_MAX (bytes) lowers the threshold (tuning knob:
-    // a large image takes L1 capacity away from the per-thread frames of big models)
-    size_t lim = 200 * 1024;
-    if (const char* s_ = getenv("TLAG_CODE_SMEM_MAX")) { const long v = atol(s_); if (v >= 0 && (size_t)v < lim) lim = (size_t)v; }
-    // Big frames (container models such as raft) are bound by local-memory latency (ncu: long-scoreboard 37 per issue,
-    // 16 warps/SM): they run with the image in global memory (read through L1) so that two CTAs fit per SM.
-    if (m->frame_words > 512 && !getenv("TLAG_CODE_SMEM_FORCE")) lim = 0;
-    e->p.code_in_smem = ((size_t)m->code_len * 8 <= lim) ? 1 : 0;
-  }
+  // bytecode image in shared memory when it fits.  Big frames (container models such as raft) are bound by local-memory
+  // latency (ncu: long-scoreboard 37 per issue, 16 warps/SM): they run with the image in global memory (read through L1)
+  // so that two CTAs fit per SM.
+  const size_t smem_lim = m->frame_words > 512 ? 0 : 200 * 1024;
+  e->p.code_in_smem = ((size_t)m->code_len * 8 <= smem_lim) ? 1 : 0;
   e->p.cpool = e->d_cpool; e->p.layout = e->d_layout; e->p.n_slots = (int)m->n_slots;
   e->p.entry_inv = m->entry_inv; e->p.entry_next = m->entry_next;
   e->p.n_off = 0; e->p.p_off = m->unpacked_words; e->p.W = (int)m->words_per_state;
@@ -1147,31 +1144,6 @@ extern "C" int tlag_create(const tlag_model* m, tlag_engine** out) {
   point_appends(e);
   e->p.ctr = e->d_ctr; e->p.flags = m->flags; e->p.n_inv = (int)m->n_invariants;
   e->p.n_ranks = 1; e->p.rank = 0; e->p.owner_words = 2;
-  // Sliced build: a successor whose packed words equal its parent's is counted (generated, has-a-successor) and dropped
-  // before the fingerprint and the seen-set probe, which would always find the parent there.  Paxos' enabled-but-
-  // unchanging actions make 65 % of its successors self-loops.  TLAG_SL_SKIPSELF=0 probes them like any other successor.
-  {
-    const char* s_ = getenv("TLAG_SL_SKIPSELF");
-    e->p.skip_self = (s_ && *s_) ? (atoi(s_) != 0) : 1;
-  }
-  // Sliced build, scalar form: successors are staged per warp and probed by the whole warp together (tlag_dev.cuh,
-  // TLAG_SL_STAGED).  TLAG_SL_STAGE=n caps the slots a warp uses below the compiled number, so that a test can make the
-  // buffer fill up and the direct path run (0: every successor is probed where it is produced).  Not a tuning knob.
-  {
-    const char* s_ = getenv("TLAG_SL_STAGE");
-    e->p.stage = (s_ && *s_) ? (atoi(s_) > 0 ? atoi(s_) : 0) : INT_MAX;
-  }
-  // TLAG_RSET_SLOTS=n starts the clustering pass's rank set at n slots (rounded up to a power of two) on every level,
-  // so that a test can make it fill up and grow.  Not a tuning knob.
-  {
-    const char* s_ = getenv("TLAG_RSET_SLOTS");
-    if (s_ && *s_) {
-      const long n = atol(s_);
-      e->rset_log2 = 1;
-      while (e->rset_log2 < 40 && (1L << e->rset_log2) < n) ++e->rset_log2;
-      e->rset_fixed = true;
-    }
-  }
   unsigned log2 = m->table_slots_log2 ? m->table_slots_log2 : 22;
   int r = alloc_table(e, log2);
   if (r) return r;

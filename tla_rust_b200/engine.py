@@ -94,7 +94,6 @@ def load_library():
     return _LIB
 
 
-FRAME_CLASSES = (64, 128, 256, 512, 1024, 2048, 4096, 8192)     # csrc/tlag_engine.cu: kFrameClasses
 NATIVE_DIR = os.path.join(_HERE, "csrc", "native")
 _NATIVE_LIBS = {}
 
