@@ -118,6 +118,52 @@ void tlag_destroy(tlag_engine *e);
 const char *tlag_last_error(const tlag_engine *e);
 const char *tlag_version(void);
 
+/* ---- random simulation (tlc -simulate) ------------------------------------------------------------------------------
+ * Walk w (a global id) of a run with seed S starts at the distinct initial state R(S, w, 0, 0xFFFFFFFF) mod n_init
+ * (distinct seeded states, first occurrence order).  At step t it checks every invariant on its state s_t, enumerates
+ * the successors of s_t in program order, and picks one of the candidates (the successors the search would store) by
+ * reservoir sampling: candidate j replaces the pick iff R(S, w, t, j) mod (j + 1) == 0.  R is tlag_sim_draw
+ * (csrc/tlag_vm.h).  A behaviour has at most `depth` states; its last state's invariants are checked, its successors
+ * are not enumerated.  A walk ends at an error, at a state without successors (a deadlock when flags has
+ * TLAG_F_DEADLOCK_CHECK), at a state whose successors are none of them candidates, or at its last state.
+ * Walks run in batches of batch_walks ids, a function of W, depth and num_walks only (tlag_sim_batch in
+ * csrc/tlag_vm.h); the run stops after the first batch
+ * that holds an error, and the error reported is the one at the smallest step, then the smallest walk id, so the
+ * result depends on (seed, first_walk, num_walks, depth) only.  The interpreter library and a model's simulation
+ * library (sliced build with simulation kernels) run it; any other library returns TLAG_EINVAL. */
+typedef struct {
+  uint64_t seed;
+  uint64_t first_walk;           /* global id of the first walk                                 */
+  uint64_t num_walks;
+  uint32_t depth;                /* states per behaviour at most (1..10^6)                      */
+  uint32_t flags;                /* TLAG_F_DEADLOCK_CHECK                                       */
+} tlag_sim_params;
+
+typedef struct {
+  int32_t  verdict;              /* TLAG_V_OK or the first error's TLAG_V_*                     */
+  int32_t  detail, detail2;      /* as in tlag_result                                           */
+  int32_t  reserved;
+  uint64_t walk, step;           /* the first error: walk id and step (0 = the initial state)   */
+  uint64_t checked;              /* states whose invariants were evaluated                      */
+  uint64_t generated;            /* successors enumerated, duplicates and non-candidates included */
+  uint64_t behaviours;           /* walks run (all of the batch that held the error)            */
+  uint64_t batch_walks;          /* walks per batch                                             */
+  double   device_ms;            /* device time of the batches (CUDA events)                    */
+} tlag_sim_result;
+
+int  tlag_simulate(tlag_engine *e, const tlag_sim_params *params, tlag_sim_result *out);
+/* The behaviour of `walk` (in the last batch run): len states (W words each, initial state first) and the action id
+ * of each (entry 0 is -1).  *len_inout: capacity in, length out (the states whose invariants were checked). */
+int  tlag_sim_trace(tlag_engine *e, uint64_t walk, uint32_t *states_out, int32_t *actions_out, uint32_t *len_inout);
+/* The history of walks [walk, walk + n) of the last batch: states_out depth x n x W words (row t = step t), actions_out
+ * depth x n ids, len_out n lengths.  Rows at or past a walk's length hold no state of its behaviour.  Any output may be
+ * NULL. */
+int  tlag_sim_read(tlag_engine *e, uint64_t walk, uint64_t n, uint32_t *states_out, int16_t *actions_out,
+                   uint32_t *len_out);
+/* XOR and SUM over the last batch of one term per state checked, from its fingerprint, walk, step and action
+ * (tlag_sim_term in csrc/tlag_vm.h). */
+int  tlag_sim_digest(tlag_engine *e, uint64_t *xor_out, uint64_t *sum_out);
+
 /* ---- multi-GPU building blocks (one engine per rank; the host exchanges the buffers,
  *      e.g. torch.distributed all_to_all_single over NCCL/NVLink; SURVEY.md §8e) ---------- */
 /* Expand the current frontier WITHOUT inserting: successor records (W state words + parent

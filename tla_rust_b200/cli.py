@@ -48,10 +48,12 @@ def pcal2tla_main(argv=None):
 
 
 def check_file(path, deadlock=True, cfg_path=None, out=None, device=0, seq_cap=None, verbose=True, lib_dirs=(),
-               engine="auto", max_depth=0):
+               engine="auto", max_depth=0, simulate=None):
     """engine: "interp" = bytecode interpreter kernel, "sliced" = the model compiled to one CUDA kernel per slice of its
     program (nvcc at run time, cached in csrc/native/), "auto" = sliced for programs big enough to repay the compile.
-    max_depth = L: stop after level L exists (levels 1..L-1 expanded) and report the prefix."""
+    max_depth = L: stop after level L exists (levels 1..L-1 expanded) and report the prefix.
+    simulate = (num, seed): random simulation instead of the search, num behaviours of at most max_depth states (100 when
+    0) from the given seed (include/tlag.h: tlag_simulate)."""
     from .checker import compile_model, encode_states, result_from_engine
     from .engine import Engine
     t0 = time.time()
@@ -95,6 +97,18 @@ def check_file(path, deadlock=True, cfg_path=None, out=None, device=0, seq_cap=N
             native = "sliced" if (engine == "sliced" or (engine == "auto" and len(cm.code) >= AUTO_SLICED_MIN_CODE)) else False
             if native == "sliced" and verbose:
                 print("Compiling the model to sm_90a kernels (one per invariant / disjunct of Next) ...", file=out)
+            if simulate is not None:
+                e = Engine(cm, deadlock=deadlock and m.check_deadlock, device=device, native=native, simulate=True)
+                e.seed(iw)
+                r = e.simulate(simulate[1], simulate[0], max_depth or 100)
+                if r["verdict"] == 4 and r["detail"] == 2 and attempt < 3:
+                    _types.SPARSE_CAP *= 2
+                    seq_cap = 2 * (seq_cap or getattr(cm, "seq_cap", None) or 4)
+                    print(f"Note: a default container capacity was exceeded; retrying with sparse capacity "
+                          f"{_types.SPARSE_CAP} and sequence capacity {seq_cap}.", file=out)
+                    e.close()
+                    continue
+                break
             world = int(os.environ.get("WORLD_SIZE", "1"))
             if world > 1:                   # `tlc -gpus N`: this process is one rank of N (see tlc_main)
                 r, trace, e = _check_distributed(cm, iw, deadlock and m.check_deadlock, native, max_depth, out)
@@ -132,6 +146,8 @@ def check_file(path, deadlock=True, cfg_path=None, out=None, device=0, seq_cap=N
             break
     finally:
         _types.SPARSE_CAP = base_sparse
+    if simulate is not None:
+        return _report_simulation(path, m, cm, r, e, simulate[1], t0, out)
     if int(os.environ.get("WORLD_SIZE", "1")) == 1:
         # The parallel search reports an error with the counts of the whole level it was found in, and with whichever of
         # several shortest behaviours won the race.  TLC's single worker stops AT the first Assert failure / deadlock
@@ -150,6 +166,14 @@ def check_file(path, deadlock=True, cfg_path=None, out=None, device=0, seq_cap=N
     res = result_from_engine(cm, r, trace)
     text = format_result(res, m.vars, m.module_name)
     print(text, file=out)
+    _write_reports(path, m, res, text)
+    print(f"Finished in {time.time() - t0:.2f}s ({r['device_seconds']:.4f}s in GPU wave kernels, "
+          f"{e.launches()} kernel launches).", file=out)
+    e.close()
+    return 0 if res.verdict == OK else 12
+
+
+def _write_reports(path, m, res, text):
     # TLC keeps its metadata (fingerprint set, trace file) under ./states/ (reference .gitignore:2); the state store of
     # this checker lives in HBM, what is worth keeping on disk is the report: states/<module>.out, and the behaviour
     # leading to an error as states/<module>.trace
@@ -170,8 +194,24 @@ def check_file(path, deadlock=True, cfg_path=None, out=None, device=0, seq_cap=N
                 os.remove(tr)
         except Exception:  # noqa: BLE001 -- the files are a convenience: never let them fail a check
             pass
-    print(f"Finished in {time.time() - t0:.2f}s ({r['device_seconds']:.4f}s in GPU wave kernels, "
-          f"{e.launches()} kernel launches).", file=out)
+
+
+def _report_simulation(path, m, cm, r, e, seed, t0, out):
+    """`tlc -simulate`: the first error's behaviour in TLC's format, or the summary; the report files as for a search"""
+    from .checker import result_from_engine
+    trace = e.sim_trace(r["walk"]) if r["verdict"] != 0 else None
+    res = result_from_engine(cm, dict(r, distinct=r["checked"], depth=len(trace[0]) if trace else 0), trace)
+    stats = (f"{r['behaviours']} behaviours simulated, {r['checked']} states checked, {r['generated']} successors "
+             f"generated (seed {seed}).")
+    if res.verdict == OK:
+        text = "Simulation completed. No error has been found.\n" + stats
+    else:
+        # the search's statistics lines do not apply: a walk has no queue and no search depth
+        text = "\n".join(format_result(res, m.vars, m.module_name).splitlines()[:-2] + [stats])
+    print(text, file=out)
+    _write_reports(path, m, res, text)
+    print(f"Finished in {time.time() - t0:.2f}s ({r['device_ms'] * 1e-3:.4f}s in GPU kernels, {e.launches()} kernel "
+          f"launches).", file=out)
     e.close()
     return 0 if res.verdict == OK else 12
 
@@ -223,6 +263,7 @@ def _free_port():
 def tlc_main(argv=None):
     argv = list(sys.argv[1:] if argv is None else argv)
     files, deadlock, cfg, dev, libs, seq_cap, engine, depth, gpus = [], True, None, 0, [], None, "auto", 0, 1
+    sim_num, seed = None, None
     i = 0
     while i < len(argv):
         a = argv[i]
@@ -240,9 +281,17 @@ def tlc_main(argv=None):
         elif a == "-engine":                # interp | sliced | auto
             i += 1
             engine = argv[i]
-        elif a == "-depth":                 # depth-bounded prefix of the breadth-first search
+        elif a == "-depth":                 # depth-bounded prefix of the breadth-first search; with -simulate: behaviour length
             i += 1
             depth = int(argv[i])
+        elif a == "-simulate":              # random behaviours instead of the search: -simulate [num=K]
+            sim_num = 1 << 20
+            if i + 1 < len(argv) and argv[i + 1].startswith("num="):
+                i += 1
+                sim_num = int(argv[i][4:])
+        elif a == "-seed":
+            i += 1
+            seed = int(argv[i])
         elif a == "-gpus":                  # partition the state space over N GPUs of this box (one process per GPU)
             i += 1
             gpus = int(argv[i])
@@ -256,8 +305,17 @@ def tlc_main(argv=None):
             files.append(a)
         i += 1
     if not files:
-        print("usage: tlc [-deadlock] [-config FILE.cfg] [-I DIR] [-seqcap N] [-engine interp|sliced|auto] [-depth N] [-gpus N] FILE.tla ...", file=sys.stderr)
+        print("usage: tlc [-deadlock] [-config FILE.cfg] [-I DIR] [-seqcap N] [-engine interp|sliced|auto] [-depth N] [-gpus N] "
+              "[-simulate [num=K] [-seed S]] FILE.tla ...", file=sys.stderr)
         return 2
+    if sim_num is not None and gpus > 1:
+        print("tlc: -simulate runs on one GPU: drop -gpus", file=sys.stderr)
+        return 2
+    if sim_num is not None and sim_num < 1:
+        print("tlc: -simulate num=K needs K >= 1", file=sys.stderr)
+        return 2
+    if sim_num is not None and seed is None:
+        seed = int.from_bytes(os.urandom(8), "little") >> 1
     if gpus > 1 and "RANK" not in os.environ:
         # re-run this command as N ranks (torch.distributed.run is plumbing: rendezvous + one process per GPU)
         import subprocess
@@ -286,9 +344,11 @@ def tlc_main(argv=None):
         if not f.endswith(".tla"):
             f += ".tla"
         print(f"Parsing file {os.path.abspath(f)}")
+        if sim_num is not None:
+            print(f"Running random simulation with seed {seed}.")
         try:
             r = check_file(f, deadlock=deadlock, cfg_path=cfg, device=dev, lib_dirs=libs, seq_cap=seq_cap,
-                           engine=engine, max_depth=depth)
+                           engine=engine, max_depth=depth, simulate=None if sim_num is None else (sim_num, seed))
         except (SpecError, ParseError, LexError, EvalError, CompileError, TypeErr) as ex:
             print(f"Error: {type(ex).__name__}: {ex}")
             r = 150

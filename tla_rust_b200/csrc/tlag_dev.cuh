@@ -52,6 +52,40 @@ struct DevParams {
   int stage;                        // sliced build, scalar form: cap on the per-warp staging slots used (0: none, all direct)
 };
 
+// ---- random simulation (tlag_simulate) ----
+// A walk's status between the kernels of a step
+enum { SIM_RUN = 0, SIM_ENDED = 1, SIM_FAILED = 2 /* this step: no successor is enumerated */,
+       SIM_FAILED_NEXT = 3 /* this step, while its successors were enumerated: the enumeration goes on */ };
+
+struct SimCtl {
+  unsigned long long stopped;       // 1 + the first step of the batch that held an error (0: none): later steps are no-ops
+  unsigned long long checked;       // states whose invariants were evaluated
+};
+
+// One step t of a batch.  The history is `depth` rows of B walks x W words; the step reads row t (DevParams::states,
+// walks [0, n)) and writes each walk's pick into row t + 1.
+struct SimParams {
+  unsigned long long seed, first;   // seed of the run, global id of the batch's walk 0
+  uint32_t t, depth, B, flags;      // step, behaviour length bound, walks per row, TLAG_F_DEADLOCK_CHECK
+  uint32_t* hist; int16_t* act;     // history rows; action id of each row's state (-1: initial)
+  uint8_t* status; uint32_t* cnt;   // per walk: SIM_*, candidates seen this step
+  uint32_t* len;                    // per walk: states checked
+  SimCtl* ctl;
+};
+
+__device__ __forceinline__ bool sim_stopped(const SimParams& s) {
+  return *(volatile const unsigned long long*)&s.ctl->stopped != 0;
+}
+
+// the pick so far of walk idx at step s.t: its successor goes to row t + 1
+__device__ __forceinline__ void sim_pick(const SimParams& s, unsigned long long idx, uint32_t j, int aid, const uint32_t* w,
+                                         int W) {
+  if (!tlag_sim_take(s.seed, s.first + idx, s.t, j)) return;
+  uint32_t* dst = s.hist + ((unsigned long long)(s.t + 1) * s.B + idx) * (unsigned long long)W;
+  for (int i = 0; i < W; ++i) dst[i] = w[i];
+  s.act[(unsigned long long)(s.t + 1) * s.B + idx] = (int16_t)aid;
+}
+
 // ---- peer-memory exchange (tlag_engine.cu: k_push / k_insert_inbox) ----
 struct P2PMeta {                       // lives in the OWNER's memory, one per source rank
   unsigned long long count[2];         // records the source pushed into buffer (seq & 1)            [written by the source]
@@ -196,7 +230,12 @@ __device__ __forceinline__ void report_min(unsigned long long* slot, unsigned lo
 // including this file, then the slice functions, then TLAG_SL_KERNEL_INV(j) / TLAG_SL_KERNEL_NEXT(j) for its slices.
 #ifdef TLAG_SLICED_DEFS
 // the scalar form's emit sites test this before they hand a successor equal to its parent to TLAG_SL_EMITW
+// (TLAG_SL_SIM, a simulation library: a self-loop is a candidate like any other successor)
+#ifdef TLAG_SL_SIM
+#define TLAG_SL_SKIPSELF 0
+#else
 #define TLAG_SL_SKIPSELF (cx->p->skip_self)
+#endif
 #include TLAG_SLICED_DEFS
 struct tlag_sl_cx {
   const DevParams* p;
@@ -207,6 +246,11 @@ struct tlag_sl_cx {
   int phase;                        // 0 = invariant slice, 1 = slice of Next
 #if TLAG_SL_SCALAR                  // (only the scalar form stages: the array form's kernels are left as they were)
   unsigned stage_cap;               // staging slots this launch may use per warp (0: every successor goes direct)
+#endif
+#ifdef TLAG_SL_SIM
+  const SimParams* sim;
+  unsigned cnt;                     // candidates of this step so far
+  int stat;                         // the walk's SIM_* status
 #endif
 };
 
@@ -228,7 +272,7 @@ static __device__ __noinline__ void sl_emit_frame(tlag_sl_cx* cx, const int32_t*
 // A slot holds the W packed words, the parent index and the meta word; at fewer than 32 slots (W > 26) nothing is staged.
 #define TLAG_SL_STAGE_BYTES 3584
 #define TLAG_SL_STAGE_SLOTS ((TLAG_SL_STAGE_BYTES / (4 * (TLAG_SL_W + 2)) / 32) * 32)
-#if TLAG_SL_SCALAR && TLAG_SL_STAGE_SLOTS >= 32
+#if TLAG_SL_SCALAR && TLAG_SL_STAGE_SLOTS >= 32 && !defined(TLAG_SL_SIM)
 #define TLAG_SL_STAGED 1
 // word-major: word k of slot s of warp v at [v][k][s], so that the lanes of an emit site (consecutive slots) and of a
 // flush (slots lane, lane + 32, ...) hit distinct banks; the row is one word longer than the slots so that the flush's
@@ -266,9 +310,18 @@ static __device__ __forceinline__ void sl_stage_words(tlag_sl_cx* cx, int aid, c
 #define TLAG_SL_EMITW(aid, o) sl_emit_words(cx, (aid), (o))
 #endif
 #define TLAG_SL_GEN() do { cx->nsucc++; cx->gen++; } while (0)
+#ifdef TLAG_SL_SIM
+// as below, and the walk fails at this step (an Assert while Next is enumerated lets the enumeration go on, as the
+// interpreter does)
+#define TLAG_SL_SIM_FAIL() (cx->stat = cx->phase == 0 ? SIM_FAILED : (cx->stat == SIM_RUN ? SIM_FAILED_NEXT : cx->stat))
+#define TLAG_SL_ASSERT(id) do { report_min(&cx->p->ctr->viol_assert, (cx->idx << 20) | (unsigned)((id) & 0xFFFFF)); TLAG_SL_SIM_FAIL(); } while (0)
+#define TLAG_SL_INVF(i) do { if (cx->phase == 0) { report_min(&cx->p->ctr->viol_inv, (cx->idx << 20) | (unsigned)((i) & 0xFFFFF)); cx->stat = SIM_FAILED; } } while (0)
+#define TLAG_SL_TRAP(code, line) do { report_min(&cx->p->ctr->viol_trap, (cx->idx << 20) | ((unsigned long long)((code) & 15) << 16) | (unsigned)((line) & 0xFFFF)); cx->nsucc++; cx->stat = SIM_FAILED; } while (0)
+#else
 #define TLAG_SL_ASSERT(id) report_min(&cx->p->ctr->viol_assert, (cx->idx << 20) | (unsigned)((id) & 0xFFFFF))
 #define TLAG_SL_INVF(i) do { if (cx->phase == 0) report_min(&cx->p->ctr->viol_inv, (cx->idx << 20) | (unsigned)((i) & 0xFFFFF)); } while (0)
 #define TLAG_SL_TRAP(code, line) do { report_min(&cx->p->ctr->viol_trap, (cx->idx << 20) | ((unsigned long long)((code) & 15) << 16) | (unsigned)((line) & 0xFFFF)); cx->nsucc++; } while (0)
+#endif
 #define TLAG_SL_SUBQ static __device__ __noinline__
 // Array form with a big frame (container models): the slice is a function of its own that receives the frame as a
 // pointer -- inlined, cicc tries scalar replacement of a 2 K-word array over a goto graph and takes many minutes (raft).

@@ -2,6 +2,13 @@
 // by a slice translation unit AFTER tlag_dev.cuh; defines the successor handling and the per-slice kernel macros.
 #pragma once
 
+#ifdef TLAG_SL_SIM
+// simulation: the successor is the step's next candidate of the walk's reservoir pick
+static __device__ __noinline__ void sl_emit_words(tlag_sl_cx* cx, int aid, const uint32_t* o) {
+  cx->nsucc++; cx->gen++;
+  sim_pick(*cx->sim, cx->idx, cx->cnt++, aid, o, TLAG_SL_W);
+}
+#else
 // successor already packed: fingerprint -> seen-set (or owner's send region) -> store
 static __device__ __noinline__ void sl_emit_words(tlag_sl_cx* cx, int aid, const uint32_t* o) {
   const DevParams& p = *cx->p;
@@ -21,6 +28,7 @@ static __device__ __noinline__ void sl_emit_words(tlag_sl_cx* cx, int aid, const
     route_append(p, w, W, fp, owner, (uint32_t)cx->idx, tlag_meta(aid, p.rank));
   }
 }
+#endif
 
 // array form: pack the primed frame (all slots, or the dirty ranges over a copy of the parent) first
 static __device__ __noinline__ void sl_emit_frame(tlag_sl_cx* cx, const int32_t* f, int aid, int dirty) {
@@ -38,6 +46,9 @@ static __device__ __noinline__ void sl_emit_frame(tlag_sl_cx* cx, const int32_t*
   if (ov) {
     cx->nsucc++; cx->gen++;
     report_min(&p.ctr->viol_trap, (cx->idx << 20) | (2ULL << 16) | (unsigned)((ov - 1) & 0xFFFF));
+#ifdef TLAG_SL_SIM
+    cx->stat = SIM_FAILED;
+#endif
     return;
   }
   // (no self-loop test here: comparing every word with the parent's row in memory cost raft 1 % of its wave time and
@@ -163,6 +174,62 @@ __device__ __forceinline__ void sl_run(const DevParams& p, unsigned long long lo
   }
 }
 
+#ifdef TLAG_SL_SIM
+// Simulation: step s.t of a batch, one thread per walk of row t (p.states).  Ended walks are skipped, and so are walks
+// that failed this step's invariants when Next runs; the reservoir count goes from one slice kernel to the next in
+// s.cnt.  The slices run in program order, so the candidates come in the interpreter's order.
+template <int PHASE, typename FN>
+__device__ __forceinline__ void sl_sim_run(const DevParams& p, const SimParams& s, unsigned long long hi, FN fn) {
+  constexpr int W = TLAG_SL_W;
+  if (sim_stopped(s) || (PHASE == 1 && s.t + 1 >= s.depth)) return;
+  tlag_sl_cx cxs;
+  tlag_sl_cx* cx = &cxs;
+  cx->p = &p; cx->sim = &s; cx->gen = 0; cx->phase = PHASE;
+  const unsigned long long stride = (unsigned long long)gridDim.x * blockDim.x;
+  for (unsigned long long idx = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; idx < hi; idx += stride) {
+    const int st = s.status[idx];
+    if (st == SIM_ENDED || (PHASE == 1 && st == SIM_FAILED)) continue;
+    const uint32_t* src = p.states + idx * (unsigned long long)W;
+    cx->idx = idx; cx->nsucc = 0; cx->stat = st; cx->cnt = PHASE == 1 ? s.cnt[idx] : 0u;
+    uint32_t in_[W];
+#pragma unroll
+    for (int i = 0; i < W; ++i) in_[i] = src[i];
+    cx->src = src;
+    fn(p.cpool, in_, cx);
+    if (cx->stat != st) s.status[idx] = (uint8_t)cx->stat;
+    if (PHASE == 1) {
+      s.cnt[idx] = cx->cnt;
+      if (cx->nsucc) p.succ_flag[idx] = 1;
+    }
+  }
+  unsigned long long g = cx->gen;
+  if (PHASE == 1) {
+    for (int o = 16; o > 0; o >>= 1) g += __shfl_down_sync(0xffffffffu, g, o);
+    if ((threadIdx.x & 31) == 0 && g) atomicAdd(&p.ctr->generated, g);
+  }
+}
+
+#define TLAG_SL_KERNEL_INV(j)                                                                                      \
+  __global__ void __launch_bounds__(TLAG_SL_BLOCK, TLAG_SL_OCC) k_sl_sim_inv_##j(                                  \
+      const __grid_constant__ DevParams p, const __grid_constant__ SimParams s, unsigned long long hi) {            \
+    sl_sim_run<0>(p, s, hi, [](const int32_t* cp, const uint32_t* f, tlag_sl_cx* cx) { tlag_sl_inv_##j(cp, f, cx); }); \
+  }
+#define TLAG_SL_KERNEL_NEXT(j)                                                                                     \
+  __global__ void __launch_bounds__(TLAG_SL_BLOCK, TLAG_SL_OCC) k_sl_sim_next_##j(                                 \
+      const __grid_constant__ DevParams p, const __grid_constant__ SimParams s, unsigned long long hi) {            \
+    sl_sim_run<1>(p, s, hi, [](const int32_t* cp, const uint32_t* f, tlag_sl_cx* cx) { tlag_sl_next_##j(cp, f, cx); }); \
+  }
+#define TLAG_SL_LAUNCH_INV(j)                                                                                      \
+  extern "C" void tlag_sl_sim_launch_inv_##j(const DevParams* p, const SimParams* s, unsigned long long hi,         \
+                                             unsigned blocks, cudaStream_t st) {                                   \
+    k_sl_sim_inv_##j<<<blocks, TLAG_SL_BLOCK, 0, st>>>(*p, *s, hi);                                                \
+  }
+#define TLAG_SL_LAUNCH_NEXT(j)                                                                                     \
+  extern "C" void tlag_sl_sim_launch_next_##j(const DevParams* p, const SimParams* s, unsigned long long hi,        \
+                                              unsigned blocks, cudaStream_t st) {                                  \
+    k_sl_sim_next_##j<<<blocks, TLAG_SL_BLOCK, 0, st>>>(*p, *s, hi);                                               \
+  }
+#else
 #define TLAG_SL_FARG const uint32_t*
 #define TLAG_SL_KERNEL_INV(j)                                                                                     \
   __global__ void __launch_bounds__(TLAG_SL_BLOCK, TLAG_SL_OCC) k_sl_inv_##j(const __grid_constant__ DevParams p, \
@@ -182,3 +249,4 @@ __device__ __forceinline__ void sl_run(const DevParams& p, unsigned long long lo
 #define TLAG_SL_LAUNCH_NEXT(j)                                                                                     \
   extern "C" void tlag_sl_launch_next_##j(const DevParams* p, unsigned long long lo, unsigned long long hi, unsigned blocks, \
                                           cudaStream_t st) { k_sl_next_##j<<<blocks, TLAG_SL_BLOCK, 0, st>>>(*p, lo, hi); }
+#endif  // TLAG_SL_SIM

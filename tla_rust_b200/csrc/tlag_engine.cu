@@ -19,6 +19,7 @@
 #include <string.h>
 #include <stdlib.h>
 #include <string>
+#include <unordered_set>
 #include <vector>
 #include <cub/device/device_radix_sort.cuh>   // CUDA-toolkit header library; used only to reorder a level (not on the hot path)
 
@@ -98,6 +99,11 @@ struct tlag_engine {
   int kg_verdict = 0, kg_detail = 0, kg_detail2 = 0; uint64_t kg_idx = 0;
   std::string err;
   uint32_t* d_scratch = nullptr; uint64_t scratch_words = 0; uint8_t* d_flags = nullptr; uint64_t flags_cap = 0;
+  // random simulation (tlag_simulate): one batch's history and per-walk state, sized for sim_B walks x sim_D rows; the
+  // last batch run stays readable (tlag_sim_trace, tlag_sim_read) until the next call
+  uint32_t* d_hist = nullptr; int16_t* d_act = nullptr; uint8_t* d_sstat = nullptr; uint8_t* d_ssucc = nullptr;
+  uint32_t* d_scnt = nullptr; uint32_t* d_slen = nullptr; SimCtl* d_sctl = nullptr; uint32_t* d_sinit = nullptr;
+  uint64_t sim_B = 0, sim_D = 0, sim_n = 0, sim_first = 0, sim_n_init = 0;
 };
 
 // ------------------------------------------------------------------ sliced native build
@@ -109,6 +115,21 @@ struct tlag_engine {
 #define TLAG_SL_BLOCK 256
 #endif
 typedef void (*sl_launch_t)(const DevParams*, unsigned long long, unsigned long long, unsigned, cudaStream_t);
+#ifdef TLAG_SL_SIM
+// a simulation library (build_sliced_library(cm, simulate=True)): its slice kernels are the simulation kernels only
+typedef void (*sl_sim_launch_t)(const DevParams*, const SimParams*, unsigned long long, unsigned, cudaStream_t);
+#define TLAG_SL_DECL_INV(j) extern "C" void tlag_sl_sim_launch_inv_##j(const DevParams*, const SimParams*, unsigned long long, unsigned, cudaStream_t);
+#define TLAG_SL_DECL_NEXT(j) extern "C" void tlag_sl_sim_launch_next_##j(const DevParams*, const SimParams*, unsigned long long, unsigned, cudaStream_t);
+TLAG_SL_INV_LIST(TLAG_SL_DECL_INV)
+TLAG_SL_NEXT_LIST(TLAG_SL_DECL_NEXT)
+#define TLAG_SL_ADDR_INV(j) tlag_sl_sim_launch_inv_##j,
+#define TLAG_SL_ADDR_NEXT(j) tlag_sl_sim_launch_next_##j,
+static const sl_sim_launch_t kSlSimInv[] = { TLAG_SL_INV_LIST(TLAG_SL_ADDR_INV) nullptr };
+static const sl_sim_launch_t kSlSimNext[] = { TLAG_SL_NEXT_LIST(TLAG_SL_ADDR_NEXT) nullptr };
+static const sl_launch_t kSlInv[] = { nullptr };
+static const sl_launch_t kSlNext[] = { nullptr };
+#define TLAG_NO_BFS(e) do { (e)->err = "this library holds the model's simulation kernels only: a search needs its BFS library"; return TLAG_EINVAL; } while (0)
+#else
 #define TLAG_SL_DECL_INV(j) extern "C" void tlag_sl_launch_inv_##j(const DevParams*, unsigned long long, unsigned long long, unsigned, cudaStream_t);
 #define TLAG_SL_DECL_NEXT(j) extern "C" void tlag_sl_launch_next_##j(const DevParams*, unsigned long long, unsigned long long, unsigned, cudaStream_t);
 TLAG_SL_INV_LIST(TLAG_SL_DECL_INV)
@@ -117,6 +138,7 @@ TLAG_SL_NEXT_LIST(TLAG_SL_DECL_NEXT)
 #define TLAG_SL_ADDR_NEXT(j) tlag_sl_launch_next_##j,
 static const sl_launch_t kSlInv[] = { TLAG_SL_INV_LIST(TLAG_SL_ADDR_INV) nullptr };
 static const sl_launch_t kSlNext[] = { TLAG_SL_NEXT_LIST(TLAG_SL_ADDR_NEXT) nullptr };
+#endif
 
 // deadlock = a frontier state for which no slice of Next produced a successor
 __global__ void k_sl_deadlock(DevParams p, unsigned long long lo, unsigned long long hi) {
@@ -267,7 +289,151 @@ k_wave(DevParams p, unsigned long long lo, unsigned long long hi) {
   if (lane == 0 && gen_local) atomicAdd(&p.ctr->generated, gen_local);
 }
 
+// ------------------------------------------------------------------ random simulation, interpreter
+// Step s.t of a batch: one lane per walk of row t (p.states, walks [0, hi)), the warp-scheduled interpreter of k_wave.
+// The invariant program runs first; at its HALT a walk that has not failed and is not at its last state runs Next, in
+// which every EMIT is packed and offered to the walk's reservoir pick (no fingerprint, no probe, no append).
+template <int FRAME, bool SMEM, bool LEAN>
+__global__ void __launch_bounds__(TLAG_BLOCK, TLAG_WAVE_OCC(FRAME, SMEM))
+k_sim(DevParams p, SimParams s, unsigned long long hi) {
+  if (sim_stopped(s)) return;
+  extern __shared__ uint64_t s_code[];
+  if (SMEM) {
+    for (uint32_t i = threadIdx.x; i < p.code_len; i += blockDim.x) s_code[i] = p.code[i];
+    __syncthreads();
+  }
+  const uint64_t* code = p.code;
+  int32_t frame[FRAME];
+  uint32_t succ[TLAG_MAXW];
+  const unsigned lane = threadIdx.x & 31;
+  const int W = p.W;
+  const bool last = s.t + 1 >= s.depth;
+  unsigned long long gen_local = 0;
+  const unsigned long long stride = (unsigned long long)gridDim.x * blockDim.x;
+  for (unsigned long long base = (unsigned long long)blockIdx.x * blockDim.x + (threadIdx.x & ~31u); base < hi; base += stride) {
+    const unsigned long long idx = base + lane;
+    int stat = idx < hi ? s.status[idx] : SIM_ENDED;
+    const bool active = stat != SIM_ENDED;
+    if (active) {
+      const uint32_t* src = p.states + idx * (unsigned long long)W;
+      for (int i = 0; i < W; ++i) succ[i] = src[i];
+      tlag_unpack(p.layout, p.n_slots, succ, frame + p.n_off);
+    }
+    int st, ev = 0;
+    int32_t info = 0, info2 = 0;
+    uint32_t pc, rpc = 0;
+    int phase = p.n_inv > 0 ? 0 : 1;
+    st = active && (phase == 0 || !last) ? L_RUN : L_DONE;
+    pc = st == L_RUN ? (phase == 0 ? p.entry_inv : p.entry_next) : TLAG_PC_PARKED;
+    unsigned nsucc = 0, cnt = 0;
+    for (;;) {
+      warp_vm<SMEM, LEAN>(code, s_code, p.cpool, frame, pc, rpc, ev, info, info2);
+      if (st == L_RUN) {
+        if (ev == TLAG_EV_EMIT) { st = L_EMIT; ++nsucc; ++gen_local; }
+        else if (ev == TLAG_EV_HALT) {
+          if (phase == 0 && !last && stat != SIM_FAILED) { phase = 1; pc = p.entry_next; } else st = L_DONE;
+        }
+        else if (ev == TLAG_EV_GEN) { ++nsucc; ++gen_local; pc = rpc; }
+        else if (ev == TLAG_EV_INVF) {
+          if (phase == 0) { report_min(&p.ctr->viol_inv, (idx << 20) | (unsigned)(info & 0xFFFFF)); stat = SIM_FAILED; }
+          pc = rpc;
+        }
+        else if (ev == TLAG_EV_ASSERT) {
+          report_min(&p.ctr->viol_assert, (idx << 20) | (unsigned)(info & 0xFFFFF));
+          stat = phase == 0 ? SIM_FAILED : (stat == SIM_RUN ? SIM_FAILED_NEXT : stat);
+          pc = rpc;
+        }
+        else {
+          report_min(&p.ctr->viol_trap, (idx << 20) | ((unsigned long long)(info & 15) << 16) | (unsigned)(info2 & 0xFFFF));
+          st = L_DONE; stat = SIM_FAILED;
+        }
+      }
+      if (__any_sync(0xffffffffu, pc != TLAG_PC_PARKED)) continue;
+      if (!__any_sync(0xffffffffu, st == L_EMIT)) break;
+      if (st == L_EMIT) {
+        int ov;
+        if (!LEAN && info2 > 0) {
+          const uint32_t* src = p.states + idx * (unsigned long long)W;
+          for (int i = 0; i < W; ++i) succ[i] = src[i];
+          ov = tlag_pack_ranges(p.layout, p.cpool, info2, frame + p.p_off, succ);
+        } else {
+          ov = tlag_pack(p.layout, p.n_slots, frame + p.p_off, succ, W);
+        }
+        if (ov) {
+          report_min(&p.ctr->viol_trap, (idx << 20) | (2ULL << 16) | (unsigned)((ov - 1) & 0xFFFF));
+          stat = SIM_FAILED;
+        } else {
+          sim_pick(s, idx, cnt++, info, succ, W);
+        }
+        st = L_RUN; pc = rpc;
+      }
+    }
+    if (active) {
+      if (stat != s.status[idx]) s.status[idx] = (uint8_t)stat;
+      s.cnt[idx] = cnt;
+      if (nsucc) p.succ_flag[idx] = 1;
+    }
+  }
+  for (int o = 16; o > 0; o >>= 1) gen_local += __shfl_down_sync(0xffffffffu, gen_local, o);
+  if (lane == 0 && gen_local) atomicAdd(&p.ctr->generated, gen_local);
+}
 #endif  // !TLAG_SLICED_INC
+
+// ------------------------------------------------------------------ random simulation, both engines
+// Each walk of the batch picks its initial state: the draw for "candidate" 0xFFFFFFFF of step 0, over the distinct
+// initial states in the order the caller seeded them.
+__global__ void k_sim_init(SimParams s, const uint32_t* __restrict__ init, unsigned long long n_init, int W,
+                           unsigned long long n) {
+  const unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const unsigned long long k = tlag_sim_draw(s.seed, s.first + i, 0, 0xFFFFFFFFu) % n_init;
+  for (int c = 0; c < W; ++c) s.hist[i * W + c] = init[k * W + c];
+  s.act[i] = -1;
+  s.status[i] = SIM_RUN; s.cnt[i] = 0; s.len[i] = 0;
+}
+
+// End of step s.t: every walk that ran it has checked one more state.  A walk that failed ends, and so does one at its
+// last state, one without successors (a deadlock when that is checked) and one whose successors were none of them
+// candidates.  Any error makes this the batch's last step (SimCtl::stopped); the others keep their pick in row t + 1.
+__global__ void k_sim_end(DevParams p, SimParams s, unsigned long long n) {
+  const unsigned long long stopped = *(volatile unsigned long long*)&s.ctl->stopped;
+  if (stopped && stopped != s.t + 1ULL) return;
+  const unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
+  unsigned long long ran = 0;
+  if (i < n && s.status[i] != SIM_ENDED) {
+    ran = 1;
+    s.len[i] = s.t + 1;
+    bool err = s.status[i] != SIM_RUN, more = false;
+    if (!err && s.t + 1 < s.depth) {
+      if (!p.succ_flag[i]) {
+        if (s.flags & TLAG_F_DEADLOCK_CHECK) { report_min(&p.ctr->viol_deadlock, i << 20); err = true; }
+      } else {
+        more = s.cnt[i] != 0;
+      }
+    }
+    if (err) atomicExch(&s.ctl->stopped, s.t + 1ULL);
+    s.status[i] = more ? SIM_RUN : SIM_ENDED;
+    s.cnt[i] = 0; p.succ_flag[i] = 0;
+  }
+  for (int o = 16; o > 0; o >>= 1) ran += __shfl_down_sync(0xffffffffu, ran, o);
+  if ((threadIdx.x & 31) == 0 && ran) atomicAdd(&s.ctl->checked, ran);
+}
+
+// XOR and SUM over the batch's behaviours: one term per state checked, from its fingerprint, walk, step and action
+__global__ void k_sim_digest(SimParams s, int W, unsigned long long n, unsigned long long* out2) {
+  unsigned long long x = 0, sm = 0;
+  const unsigned long long total = n * s.depth;
+  for (unsigned long long k = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; k < total;
+       k += (unsigned long long)gridDim.x * blockDim.x) {
+    const unsigned long long i = k % n, t = k / n;
+    if (t >= s.len[i]) continue;
+    const unsigned long long v = tlag_sim_term(tlag_fingerprint(s.hist + (t * s.B + i) * W, W), s.first + i, (uint32_t)t,
+                                               s.act[t * s.B + i]);
+    x ^= v; sm += v;
+  }
+  for (int o = 16; o > 0; o >>= 1) { x ^= __shfl_down_sync(0xffffffffu, x, o); sm += __shfl_down_sync(0xffffffffu, sm, o); }
+  if ((threadIdx.x & 31) == 0) { atomicXor(&out2[0], x); atomicAdd(&out2[1], sm); }
+}
 
 // ------------------------------------------------------------------ K1 alone: fingerprint + probe/insert
 // One thread per candidate state, word by word: the inputs the staged form does not take (W = 1, or a batch that is not
@@ -1153,10 +1319,12 @@ extern "C" int tlag_create(const tlag_model* m, tlag_engine** out) {
 
 extern "C" void tlag_destroy(tlag_engine* e) {
   if (!e) return;
-  cudaFree(e->d_code); cudaFree(e->d_cpool); cudaFree(e->d_layout); cudaFree(e->d_ctr); cudaFree(e->d_dig);
+  cudaFree(e->d_code); cudaFree(e->d_cpool); cudaFree(e->d_layout); cudaFree(e->d_ctr); cudaFree(e->d_dig); cudaFree(e->d_sctl);
   if (e->stream) {
     dfree(e, e->d_states); dfree(e, e->d_parent); dfree(e, e->d_meta); dfree(e, e->d_table);
     dfree(e, e->d_scratch); dfree(e, e->d_flags); dfree(e, e->d_disc); dfree(e, e->d_sort); dfree(e, e->d_rset); dfree(e, e->d_sent); dfree(e, e->d_succ);
+    dfree(e, e->d_hist); dfree(e, e->d_act); dfree(e, e->d_sstat); dfree(e, e->d_ssucc); dfree(e, e->d_scnt); dfree(e, e->d_slen);
+    dfree(e, e->d_sinit);
     cudaStreamSynchronize(e->stream);
   }
   if (e->p2p_slot >= 0) {                              // exchange buffers and peer mappings are parked, not released
@@ -1411,6 +1579,9 @@ static int rollback_wave(tlag_engine* e, uint64_t hi, uint64_t want_states) {
 
 extern "C" int tlag_step(tlag_engine* e, tlag_wave_stats* out) {
   if (!e) return TLAG_EINVAL;
+#ifdef TLAG_NO_BFS
+  TLAG_NO_BFS(e);
+#endif
   if (out) memset(out, 0, sizeof(*out));
   start_search(e);
   if (e->verdict != TLAG_V_RUNNING) { if (out) out->verdict = e->verdict; return TLAG_OK; }
@@ -1597,6 +1768,9 @@ extern "C" int tlag_set_rank(tlag_engine* e, uint32_t n_ranks, uint32_t rank) {
 extern "C" int tlag_expand_route(tlag_engine* e, uint32_t n_ranks, uint64_t first, uint64_t count, uint64_t d_send,
                                  uint64_t cap_records, uint64_t* counts, tlag_wave_stats* out) {
   if (!e || !counts || n_ranks == 0 || n_ranks > 16) return TLAG_EINVAL;
+#ifdef TLAG_NO_BFS
+  TLAG_NO_BFS(e);
+#endif
   if (out) memset(out, 0, sizeof(*out));
   start_search(e);
   uint64_t lo = e->lo + first, hi = lo + count;
@@ -1741,6 +1915,9 @@ extern "C" int tlag_p2p_attach(tlag_engine* e, uint32_t peer, const uint8_t* han
 extern "C" int tlag_p2p_level(tlag_engine* e, uint64_t n_chunks, uint64_t chunk_states, uint64_t expect_inbound,
                               tlag_wave_stats* out) {
   if (!e || chunk_states == 0) return TLAG_EINVAL;
+#ifdef TLAG_NO_BFS
+  TLAG_NO_BFS(e);
+#endif
   if (!e->p2p_ready && e->q.n_ranks > 1) { e->err = "tlag_p2p_level before every peer was attached"; return TLAG_ESTATE; }
   if (out) memset(out, 0, sizeof(*out));
   start_search(e);
@@ -1815,4 +1992,234 @@ extern "C" int tlag_advance_level(tlag_engine* e, tlag_wave_stats* out) {
   Counters hc;
   CK(read_counters(e, &hc));
   return close_level(e, hc.n_states, true, out);
+}
+
+// ---- random simulation (include/tlag.h: tlag_simulate) ------------------------------------------------------------
+#if defined(TLAG_SLICED_INC)
+#if defined(TLAG_SL_SIM)
+static cudaError_t launch_sim_step(tlag_engine* e, const DevParams& p, const SimParams& s, uint64_t n) {
+  uint64_t blocks = (n + TLAG_SL_BLOCK - 1) / TLAG_SL_BLOCK;
+  if (blocks > (uint64_t)e->sm_count * 64) blocks = (uint64_t)e->sm_count * 64;
+  if (p.n_inv > 0)
+    for (int j = 0; kSlSimInv[j]; ++j) { kSlSimInv[j](&p, &s, n, (unsigned)blocks, e->stream); e->launches++; }
+  for (int j = 0; kSlSimNext[j]; ++j) { kSlSimNext[j](&p, &s, n, (unsigned)blocks, e->stream); e->launches++; }
+  return cudaGetLastError();
+}
+#endif
+#else
+static cudaError_t launch_sim_step(tlag_engine* e, const DevParams& p, const SimParams& s, uint64_t n) {
+  const size_t smem = p.code_in_smem ? (size_t)p.code_len * 8 : 0;
+  void (*fn)(DevParams, SimParams, unsigned long long) = nullptr;
+  const bool sm = p.code_in_smem != 0;
+  const bool lean = !e->uses_ext;
+  switch (e->frame_class) {
+    case 0: fn = lean ? (sm ? k_sim<64, true, true> : k_sim<64, false, true>) : (sm ? k_sim<64, true, false> : k_sim<64, false, false>); break;
+    case 1: fn = lean ? (sm ? k_sim<128, true, true> : k_sim<128, false, true>) : (sm ? k_sim<128, true, false> : k_sim<128, false, false>); break;
+    case 2: fn = lean ? (sm ? k_sim<256, true, true> : k_sim<256, false, true>) : (sm ? k_sim<256, true, false> : k_sim<256, false, false>); break;
+    case 3: fn = lean ? (sm ? k_sim<512, true, true> : k_sim<512, false, true>) : (sm ? k_sim<512, true, false> : k_sim<512, false, false>); break;
+    case 4: fn = sm ? k_sim<1024, true, false> : k_sim<1024, false, false>; break;
+    case 5: fn = sm ? k_sim<2048, true, false> : k_sim<2048, false, false>; break;
+    case 6: fn = sm ? k_sim<4096, true, false> : k_sim<4096, false, false>; break;
+    default: fn = sm ? k_sim<8192, true, false> : k_sim<8192, false, false>; break;
+  }
+  if (smem > 48 * 1024) {
+    cudaError_t r = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (r != cudaSuccess) return r;
+  }
+  int occ = 1;
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, fn, TLAG_BLOCK, smem) != cudaSuccess || occ < 1) occ = 1;
+  uint64_t blocks = (n + TLAG_BLOCK - 1) / TLAG_BLOCK;
+  if (blocks > (uint64_t)e->sm_count * (uint64_t)occ) blocks = (uint64_t)e->sm_count * (uint64_t)occ;
+  fn<<<(unsigned)blocks, TLAG_BLOCK, smem, e->stream>>>(p, s, n);
+  e->launches++;
+  return cudaGetLastError();
+}
+#endif
+
+#if !defined(TLAG_SLICED_INC) || defined(TLAG_SL_SIM)
+// The batch's buffers: sim_B walks x sim_D rows of history, the per-walk state, and the distinct initial states in the
+// order the caller seeded them (first occurrence)
+static int sim_buffers(tlag_engine* e, uint64_t B, uint64_t D) {
+  const uint64_t W = e->m.words_per_state;
+  if (B * D > e->sim_B * e->sim_D || B > e->sim_B) {
+    dfree(e, e->d_hist); dfree(e, e->d_act); dfree(e, e->d_sstat); dfree(e, e->d_ssucc); dfree(e, e->d_scnt); dfree(e, e->d_slen);
+    e->d_hist = nullptr; e->d_act = nullptr; e->d_sstat = e->d_ssucc = nullptr; e->d_scnt = e->d_slen = nullptr;
+    e->sim_B = e->sim_D = 0;
+    CK(dmalloc(e, &e->d_hist, B * D * W * 4));
+    CK(dmalloc(e, &e->d_act, B * D * 2));
+    CK(dmalloc(e, &e->d_sstat, B));
+    CK(dmalloc(e, &e->d_ssucc, B));
+    CK(dmalloc(e, &e->d_scnt, B * 4));
+    CK(dmalloc(e, &e->d_slen, B * 4));
+  }
+  e->sim_B = B; e->sim_D = D;
+  if (!e->d_sctl) CK(cudaMalloc(&e->d_sctl, sizeof(SimCtl)));
+  if (!e->d_sinit) {
+    std::vector<uint32_t> distinct;
+    std::unordered_set<std::string> seen;
+    const uint64_t n = e->h_init.size() / W;
+    for (uint64_t i = 0; i < n; ++i)
+      if (seen.insert(std::string((const char*)(e->h_init.data() + i * W), W * 4)).second)
+        distinct.insert(distinct.end(), e->h_init.begin() + i * W, e->h_init.begin() + (i + 1) * W);
+    e->sim_n_init = distinct.size() / W;
+    if (!e->sim_n_init) { e->err = "tlag_simulate: no initial state was seeded"; return TLAG_ESTATE; }
+    CK(dmalloc(e, &e->d_sinit, distinct.size() * 4));
+    CK(cudaMemcpyAsync(e->d_sinit, distinct.data(), distinct.size() * 4, cudaMemcpyHostToDevice, e->stream));
+    CK(cudaStreamSynchronize(e->stream));
+  }
+  return TLAG_OK;
+}
+
+static SimParams sim_params(tlag_engine* e, const tlag_sim_params* sp, uint64_t first) {
+  SimParams s;
+  memset(&s, 0, sizeof(s));
+  s.seed = sp->seed; s.first = first; s.depth = sp->depth; s.B = (uint32_t)e->sim_B; s.flags = sp->flags;
+  s.hist = e->d_hist; s.act = e->d_act; s.status = e->d_sstat; s.cnt = e->d_scnt; s.len = e->d_slen; s.ctl = e->d_sctl;
+  return s;
+}
+#endif
+
+extern "C" int tlag_simulate(tlag_engine* e, const tlag_sim_params* sp, tlag_sim_result* out) {
+  if (!e || !sp || !out) return TLAG_EINVAL;
+  memset(out, 0, sizeof(*out));
+#if defined(TLAG_SLICED_INC) && !defined(TLAG_SL_SIM)
+  e->err = "this library has no simulation kernels: build the model's simulation library (build_sliced_library(cm, simulate=True))";
+  return TLAG_EINVAL;
+#else
+  if (sp->depth < 1 || sp->depth > 1000000 || sp->num_walks == 0) { e->err = "tlag_simulate: depth must be 1..10^6 and num_walks > 0"; return TLAG_EINVAL; }
+  if (e->m.n_actions > 32767) { e->err = "tlag_simulate: more than 32767 actions"; return TLAG_EINVAL; }
+  if (sp->first_walk + sp->num_walks < sp->first_walk) { e->err = "tlag_simulate: walk ids past 2^64"; return TLAG_EINVAL; }
+  const uint64_t W = e->m.words_per_state, D = sp->depth;
+  const uint64_t B = tlag_sim_batch((uint32_t)W, sp->depth, sp->num_walks);
+  int r = sim_buffers(e, B, D);
+  if (r) return r;
+  out->verdict = TLAG_V_OK;
+  out->batch_walks = B;
+  float total_ms = 0;
+  for (uint64_t done = 0; done < sp->num_walks; done += B) {
+    const uint64_t n = sp->num_walks - done < B ? sp->num_walks - done : B, first = sp->first_walk + done;
+    e->sim_n = n; e->sim_first = first;
+    CK(reset_counters(e, 0));
+    CK(cudaMemsetAsync(e->d_sctl, 0, sizeof(SimCtl), e->stream));
+    CK(cudaMemsetAsync(e->d_ssucc, 0, n, e->stream));
+    SimParams s = sim_params(e, sp, first);
+    DevParams p = e->p;
+    p.succ_flag = e->d_ssucc;
+    Counters hc;
+    float ms = 0;
+    r = timed(e, &ms, &hc, [&] {
+      const unsigned blocks = (unsigned)((n + 255) / 256);
+      k_sim_init<<<blocks, 256, 0, e->stream>>>(s, e->d_sinit, e->sim_n_init, (int)W, n);
+      e->launches++;
+      CK(cudaGetLastError());
+      for (uint32_t t = 0; t < sp->depth; ++t) {
+        s.t = t;
+        p.states = e->d_hist + (uint64_t)t * B * W;
+        CK(launch_sim_step(e, p, s, n));
+        k_sim_end<<<blocks, 256, 0, e->stream>>>(p, s, n);
+        e->launches++;
+        CK(cudaGetLastError());
+      }
+      return TLAG_OK;
+    });
+    if (r) return r;
+    total_ms += ms;
+    SimCtl hs;
+    CK(cudaMemcpy(&hs, e->d_sctl, sizeof(hs), cudaMemcpyDeviceToHost));
+    out->generated += hc.generated;
+    out->checked += hs.checked;
+    out->behaviours += n;
+    if (hs.stopped) {
+      const int saved = e->verdict;
+      collect_violations(e, hc);
+      out->verdict = e->verdict; out->detail = e->detail; out->detail2 = e->detail2;
+      out->walk = first + e->viol_idx; out->step = hs.stopped - 1;
+      e->verdict = saved;
+      break;
+    }
+  }
+  out->device_ms = total_ms;
+  return TLAG_OK;
+#endif
+}
+
+#if !defined(TLAG_SLICED_INC) || defined(TLAG_SL_SIM)
+// walk (a global id) -> its column in the last batch
+static int sim_column(tlag_engine* e, uint64_t walk, uint64_t n, uint64_t* col) {
+  if (!e->sim_n || walk < e->sim_first || walk + n > e->sim_first + e->sim_n || walk + n < walk) {
+    e->err = "no such walk in the last batch of tlag_simulate";
+    return TLAG_EINVAL;
+  }
+  *col = walk - e->sim_first;
+  return TLAG_OK;
+}
+#endif
+
+extern "C" int tlag_sim_read(tlag_engine* e, uint64_t walk, uint64_t n, uint32_t* states_out, int16_t* actions_out,
+                             uint32_t* len_out) {
+  if (!e) return TLAG_EINVAL;
+#if defined(TLAG_SLICED_INC) && !defined(TLAG_SL_SIM)
+  e->err = "this library has no simulation kernels";
+  return TLAG_EINVAL;
+#else
+  uint64_t c = 0;
+  int r = sim_column(e, walk, n, &c);
+  if (r) return r;
+  const uint64_t W = e->m.words_per_state, B = e->sim_B, D = e->sim_D;
+  if (states_out)
+    CK(cudaMemcpy2DAsync(states_out, n * W * 4, e->d_hist + c * W, B * W * 4, n * W * 4, D, cudaMemcpyDeviceToHost, e->stream));
+  if (actions_out)
+    CK(cudaMemcpy2DAsync(actions_out, n * 2, e->d_act + c, B * 2, n * 2, D, cudaMemcpyDeviceToHost, e->stream));
+  if (len_out) CK(cudaMemcpyAsync(len_out, e->d_slen + c, n * 4, cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaStreamSynchronize(e->stream));
+  return TLAG_OK;
+#endif
+}
+
+extern "C" int tlag_sim_trace(tlag_engine* e, uint64_t walk, uint32_t* states_out, int32_t* actions_out, uint32_t* len_inout) {
+  if (!e || !len_inout) return TLAG_EINVAL;
+#if defined(TLAG_SLICED_INC) && !defined(TLAG_SL_SIM)
+  e->err = "this library has no simulation kernels";
+  return TLAG_EINVAL;
+#else
+  uint64_t c = 0;
+  int r = sim_column(e, walk, 1, &c);
+  if (r) return r;
+  const uint64_t W = e->m.words_per_state, B = e->sim_B;
+  uint32_t len = 0;
+  CK(cudaMemcpy(&len, e->d_slen + c, 4, cudaMemcpyDeviceToHost));
+  if (len > *len_inout) { *len_inout = len; e->err = "tlag_sim_trace: buffer too small"; return TLAG_EINVAL; }
+  std::vector<int16_t> a(len);
+  if (len && states_out)
+    CK(cudaMemcpy2DAsync(states_out, W * 4, e->d_hist + c * W, B * W * 4, W * 4, len, cudaMemcpyDeviceToHost, e->stream));
+  if (len) CK(cudaMemcpy2DAsync(a.data(), 2, e->d_act + c, B * 2, 2, len, cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaStreamSynchronize(e->stream));
+  if (actions_out) for (uint32_t i = 0; i < len; ++i) actions_out[i] = a[i];
+  *len_inout = len;
+  return TLAG_OK;
+#endif
+}
+
+extern "C" int tlag_sim_digest(tlag_engine* e, uint64_t* xor_out, uint64_t* sum_out) {
+  if (!e || !xor_out || !sum_out) return TLAG_EINVAL;
+#if defined(TLAG_SLICED_INC) && !defined(TLAG_SL_SIM)
+  e->err = "this library has no simulation kernels";
+  return TLAG_EINVAL;
+#else
+  if (!e->sim_n) { e->err = "tlag_sim_digest before tlag_simulate"; return TLAG_ESTATE; }
+  if (!e->d_dig) CK(cudaMalloc(&e->d_dig, 16));
+  CK(cudaMemsetAsync(e->d_dig, 0, 16, e->stream));
+  tlag_sim_params sp;
+  memset(&sp, 0, sizeof(sp));
+  sp.depth = (uint32_t)e->sim_D;
+  const SimParams s = sim_params(e, &sp, e->sim_first);
+  k_sim_digest<<<e->sm_count * 8, 256, 0, e->stream>>>(s, (int)e->m.words_per_state, e->sim_n, e->d_dig);
+  e->launches++;
+  CK(cudaGetLastError());
+  unsigned long long h2[2];
+  CK(cudaMemcpyAsync(h2, e->d_dig, 16, cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaStreamSynchronize(e->stream));
+  *xor_out = h2[0]; *sum_out = h2[1];
+  return TLAG_OK;
+#endif
 }

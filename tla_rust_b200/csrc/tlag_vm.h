@@ -181,6 +181,39 @@ TLAG_HD uint64_t tlag_fingerprint(const uint32_t* w, int W) {
   return tlag_fp_final(h, W);
 }
 
+// ---- random simulation ---------------------------------------------------------------
+// The draw of walk w (global id) of a run with seed S at step t for candidate j (j = 0xFFFFFFFF: the initial state).
+// A walk is a pure function of (S, w): the device engines and the CPU walker of the tests make the same choices.
+TLAG_HD uint64_t tlag_mix64(uint64_t z) {   // splitmix64 finaliser
+  z = (z ^ (z >> 30)) * 0xbf58476d1ce4e5b9ULL; z = (z ^ (z >> 27)) * 0x94d049bb133111ebULL; return z ^ (z >> 31);
+}
+
+TLAG_HD uint64_t tlag_sim_draw(uint64_t seed, uint64_t w, uint32_t t, uint32_t j) {
+  return tlag_mix64(tlag_mix64(tlag_mix64(seed + 0x9E3779B97F4A7C15ULL) ^ w) ^ (((uint64_t)t << 32) | (uint64_t)j));
+}
+
+// Reservoir sampling over a step's candidates: candidate j (0-based, in emission order) replaces the pick iff this holds,
+// so that each of k candidates is picked with probability 1/k.
+TLAG_HD int tlag_sim_take(uint64_t seed, uint64_t w, uint32_t t, uint32_t j) {
+  return tlag_sim_draw(seed, w, t, j) % ((uint64_t)j + 1ULL) == 0ULL;
+}
+
+// One state of a behaviour in the history digest (tlag_sim_digest): its fingerprint, walk, step and action id
+TLAG_HD uint64_t tlag_sim_term(uint64_t fp, uint64_t w, uint32_t t, int32_t act) {
+  return tlag_mix64(fp ^ tlag_mix64(w * 0x9E3779B97F4A7C15ULL + ((uint64_t)t << 16) + (uint64_t)(uint16_t)act));
+}
+
+// Walks of one batch: min(num, 2^20, what a 4 GiB history holds at depth D), rounded down to a multiple of 32 (at least
+// 32).  It depends on W, D and num only, so a run's batches, and with them its first error, are the same on any GPU.
+#define TLAG_SIM_BUDGET (4ULL << 30)
+TLAG_HD uint64_t tlag_sim_batch(uint32_t W, uint32_t D, uint64_t num) {
+  uint64_t b = TLAG_SIM_BUDGET / ((uint64_t)D * (4ULL * W + 2ULL));
+  if (b > (1ULL << 20)) b = 1ULL << 20;
+  if (b > num) b = num;
+  b &= ~31ULL;
+  return b < 32 ? 32 : b;
+}
+
 // ---- multi-GPU ownership ---------------------------------------------------------
 // Owner rank of a state = hash of its LAST TWO packed words (the clustering key of the frontier sort)
 // scaled to n_ranks.  All states of one cluster therefore live on, and are expanded by, the same rank, so a

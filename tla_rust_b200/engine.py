@@ -61,11 +61,26 @@ class TlagResult(C.Structure):
         return {f: getattr(self, f) for f, _ in self._fields_}
 
 
+class SimParams(C.Structure):
+    _fields_ = [("seed", C.c_uint64), ("first_walk", C.c_uint64), ("num_walks", C.c_uint64), ("depth", C.c_uint32),
+                ("flags", C.c_uint32)]
+
+
+class SimResult(C.Structure):
+    _fields_ = [("verdict", C.c_int32), ("detail", C.c_int32), ("detail2", C.c_int32), ("reserved", C.c_int32),
+                ("walk", C.c_uint64), ("step", C.c_uint64), ("checked", C.c_uint64), ("generated", C.c_uint64),
+                ("behaviours", C.c_uint64), ("batch_walks", C.c_uint64), ("device_ms", C.c_double)]
+
+    def as_dict(self):
+        return {f: getattr(self, f) for f, _ in self._fields_}
+
+
 EXPORTS = ["tlag_create", "tlag_seed", "tlag_step", "tlag_run", "tlag_result_now", "tlag_trace",
            "tlag_read_states", "tlag_digest", "tlag_probe_batch", "tlag_probe_batch_device", "tlag_reset_table", "tlag_restart",
            "tlag_kernel_launches", "tlag_destroy", "tlag_last_error", "tlag_version",
            "tlag_frontier", "tlag_expand_route", "tlag_insert_records", "tlag_advance_level",
-           "tlag_p2p_init", "tlag_p2p_attach", "tlag_p2p_level", "tlag_p2p_rollback", "tlag_read_link", "tlag_set_rank", "tlag_set_owner_words"]
+           "tlag_p2p_init", "tlag_p2p_attach", "tlag_p2p_level", "tlag_p2p_rollback", "tlag_read_link", "tlag_set_rank", "tlag_set_owner_words",
+           "tlag_simulate", "tlag_sim_trace", "tlag_sim_read", "tlag_sim_digest"]
 
 
 def build_library(verbose=False):
@@ -98,7 +113,7 @@ NATIVE_DIR = os.path.join(_HERE, "csrc", "native")
 _NATIVE_LIBS = {}
 
 
-def _sliced_tag(cm, scalar):
+def _sliced_tag(cm, scalar, simulate=False):
     import hashlib
     from .compile.sliced import model_key
     h = hashlib.sha256()
@@ -110,7 +125,7 @@ def _sliced_tag(cm, scalar):
                    os.environ.get("TLAG_SL_MIN_SLICE", ""))).encode())
     if os.environ.get("TLAG_CSRC_DIR"):                 # experiments built from a modified copy of csrc/
         h.update(os.environ["TLAG_CSRC_DIR"].encode())
-    return f"sl_{model_key(cm)}_{h.hexdigest()[:8]}{'_s' if scalar else ''}"
+    return f"sl_{model_key(cm)}_{h.hexdigest()[:8]}{'_s' if scalar else ''}{'_sim' if simulate else ''}"
 
 
 def sliced_form(cm):
@@ -128,22 +143,24 @@ def sliced_form(cm):
         return False
 
 
-def sliced_library_path(cm, scalar=None):
+def sliced_library_path(cm, scalar=None, simulate=False):
     if scalar is None:
         scalar = sliced_form(cm)
-    return os.path.join(NATIVE_DIR, f"libtlag_{_sliced_tag(cm, scalar)}.so")
+    return os.path.join(NATIVE_DIR, f"libtlag_{_sliced_tag(cm, scalar, simulate)}.so")
 
 
-def build_sliced_library(cm, force=False, verbose=False, scalar=None, jobs=None):
+def build_sliced_library(cm, force=False, verbose=False, scalar=None, jobs=None, simulate=False):
     """Model-specialised engine library, sliced form (compile/sliced.py): one kernel per invariant and per disjunct of
     Next, same engine source and C ABI.  The slices are spread over several translation units that nvcc compiles in
-    parallel (-dc) next to the engine's own unit; built in-tree (csrc/native/) so that it travels with the snapshot."""
+    parallel (-dc) next to the engine's own unit; built in-tree (csrc/native/) so that it travels with the snapshot.
+    simulate=True: the model's simulation library instead (tlag_simulate; the same slices compiled with -DTLAG_SL_SIM
+    into the simulation kernels, no BFS), a library of its own."""
     from concurrent.futures import ThreadPoolExecutor
     from .compile.sliced import emit_parts
     if scalar is None:
         scalar = sliced_form(cm)
     os.makedirs(NATIVE_DIR, exist_ok=True)
-    tag = _sliced_tag(cm, scalar)
+    tag = _sliced_tag(cm, scalar, simulate)
     so = os.path.join(NATIVE_DIR, f"libtlag_{tag}.so")
     if os.path.exists(so) and not force:
         return so
@@ -163,6 +180,8 @@ def build_sliced_library(cm, force=False, verbose=False, scalar=None, jobs=None)
     base = [nvcc, "-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", *NVCC_ARCH, "-I", csrc, "-dc"]
     if not scalar and cm.frame_words > 512:
         base.append("-DTLAG_SL_SEG_NOINLINE")
+    if simulate:
+        base.append("-DTLAG_SL_SIM")
     for k in ("TLAG_SL_OCC", "TLAG_SL_BLOCK"):
         if os.environ.get(k):
             base.append(f"-D{k}={int(os.environ[k])}")
@@ -193,15 +212,15 @@ def build_sliced_library(cm, force=False, verbose=False, scalar=None, jobs=None)
     return so
 
 
-def load_sliced_library(cm, build=True):
+def load_sliced_library(cm, build=True, simulate=False):
     if os.environ.get("TLAG_NO_BUILD") == "1":      # GPU sessions: never spend box time in nvcc
         build = False
-    so = sliced_library_path(cm)
+    so = sliced_library_path(cm, simulate=simulate)
     if so not in _NATIVE_LIBS:
         if not os.path.exists(so):
             if not build:
                 raise EngineUnavailable(f"{so} is missing (sliced native build of this model)")
-            build_sliced_library(cm)
+            build_sliced_library(cm, simulate=simulate)
         _NATIVE_LIBS[so] = _bind(so)
     return _NATIVE_LIBS[so]
 
@@ -209,16 +228,20 @@ def load_sliced_library(cm, build=True):
 class Engine:
     """One BFS engine instance on one GPU (mirrors tlag_engine)."""
 
-    def __init__(self, cm, deadlock=True, device=0, table_log2=0, max_states=0, keep_going=False, native=None, exact=False):
+    def __init__(self, cm, deadlock=True, device=0, table_log2=0, max_states=0, keep_going=False, native=None, exact=False,
+                 simulate=False):
         """native="sliced" (or True): the model-specialised sliced build -- one kernel per invariant / disjunct of Next,
         compile/sliced.py; built on demand with nvcc and cached in csrc/native/; False: the bytecode interpreter kernel;
-        None: follow the environment variable TLAG_NATIVE (sliced / 0)."""
+        None: follow the environment variable TLAG_NATIVE (sliced / 0).
+        simulate=True with the sliced build: the model's simulation library, which runs simulate() and no search (the
+        interpreter library runs both)."""
         if native is None:
             native = "sliced" if os.environ.get("TLAG_NATIVE", "0") in ("sliced", "1") else False
         if exact:               # TLAG_F_EXACT: TLC's single worker replayed on the device (interpreter kernel, one warp)
             native = False
         self.native = "sliced" if native else False
-        self.L = load_sliced_library(cm) if self.native else load_library()
+        self.deadlock = deadlock
+        self.L = load_sliced_library(cm, simulate=simulate) if self.native else load_library()
         self.cm = cm
         self._code = np.ascontiguousarray(cm.code, dtype=np.uint64)
         self._cpool = np.ascontiguousarray(cm.cpool, dtype=np.int32)
@@ -323,6 +346,46 @@ class Engine:
 
     def launches(self) -> int:
         return int(self.L.tlag_kernel_launches(self.h))
+
+    # random simulation (include/tlag.h: tlag_simulate)
+    def simulate(self, seed, num, depth, first=0) -> dict:
+        """`num` random behaviours of at most `depth` states, walks first..first + num - 1 of the run with this seed
+        (deadlocks checked as the engine was created).  -> dict(verdict, detail, detail2, walk, step, checked,
+        generated, behaviours, batch_walks, device_ms)"""
+        r = SimResult()
+        self._sim_depth = depth
+        sp = SimParams(seed & 0xFFFFFFFFFFFFFFFF, first, num, depth, F_DEADLOCK_CHECK if self.deadlock else 0)
+        self._ck(self.L.tlag_simulate(self.h, C.byref(sp), C.byref(r)), "tlag_simulate")
+        return r.as_dict()
+
+    def sim_trace(self, walk, cap=1 << 20):
+        """-> (states, action ids) of a walk of the last batch, as trace() returns them"""
+        W = self.cm.W
+        n = C.c_uint32(cap)
+        self._ck(self.L.tlag_sim_trace(self.h, C.c_uint64(walk), None, None, C.byref(n)), "tlag_sim_trace")
+        states = np.zeros((n.value, W), dtype=np.uint32)
+        acts = np.zeros(n.value, dtype=np.int32)
+        self._ck(self.L.tlag_sim_trace(self.h, C.c_uint64(walk), states.ctypes.data_as(C.c_void_p),
+                                       acts.ctypes.data_as(C.c_void_p), C.byref(n)), "tlag_sim_trace")
+        return states, acts
+
+    def sim_read(self, walk, n):
+        """History of walks [walk, walk + n) of the last batch: (states [depth, n, W], action ids [depth, n], lengths [n])"""
+        L, W = self.L, self.cm.W
+        lens = np.zeros(n, dtype=np.uint32)
+        self._ck(L.tlag_sim_read(self.h, C.c_uint64(walk), C.c_uint64(n), None, None, lens.ctypes.data_as(C.c_void_p)),
+                 "tlag_sim_read")
+        depth = self._sim_depth
+        states = np.zeros((depth, n, W), dtype=np.uint32)
+        acts = np.zeros((depth, n), dtype=np.int16)
+        self._ck(L.tlag_sim_read(self.h, C.c_uint64(walk), C.c_uint64(n), states.ctypes.data_as(C.c_void_p),
+                                 acts.ctypes.data_as(C.c_void_p), None), "tlag_sim_read")
+        return states, acts, lens
+
+    def sim_digest(self):
+        x, s_ = C.c_uint64(), C.c_uint64()
+        self._ck(self.L.tlag_sim_digest(self.h, C.byref(x), C.byref(s_)), "tlag_sim_digest")
+        return int(x.value), int(s_.value)
 
     # multi-GPU building blocks
     def frontier(self):
