@@ -164,6 +164,37 @@ int  tlag_sim_read(tlag_engine *e, uint64_t walk, uint64_t n, uint32_t *states_o
  * (tlag_sim_term in csrc/tlag_vm.h). */
 int  tlag_sim_digest(tlag_engine *e, uint64_t *xor_out, uint64_t *sum_out);
 
+/* ---- state graph (tlc -dump dot; the input of the liveness checks) ---------------------------------------------------
+ * After a search call, the state graph covers every state of the store.  Rows [0, n_expanded) are the states the search
+ * expanded; the store is level-contiguous, so n_expanded is the first row of the current frontier: n_states at the
+ * fixpoint, the first row of the first unexpanded level after a violation (the level that found it is finished), the
+ * first row of level L after a depth-bounded stop.  There is one edge (s, t, a) per distinct triple where s is an
+ * expanded row, Next enumerated from s reaches an EMIT (a successor the search would store, not a GEN) with action id a
+ * (as tlag_trace reports it), the packed successor (under SYMMETRY the representative EMIT produces) is stored row t, and
+ * t != s: self-loops are not edges (as for tlag_scc).  The same t reached by two actions makes two edges.  Edges are CSR
+ * by source row, and within a row ordered by (t, a).  The set of (fingerprint(s), fingerprint(t), a) does not depend on
+ * the store's order: both device engines and any run give the same set.
+ * tlag_build_graph builds it in device memory: an index pass maps every seen-set slot to its row (4 bytes per slot), then
+ * Next runs over chunks of expanded rows on the interpreter (the sliced libraries included) and each chunk's edges are
+ * sorted, made distinct and appended.  The clustering and discovery buffers and the routed-fingerprint cache are freed
+ * first; a graph that does not fit is TLAG_ENOMEM.  Refused: a simulation library and a TLAG_F_EXACT engine
+ * (TLAG_EINVAL), an engine that holds one shard of a multi-GPU search (tlag_set_rank with n > 1, tlag_p2p_init;
+ * TLAG_EINVAL), an engine not seeded (TLAG_ESTATE) and a search that stopped at an evaluation trap, whose successor sets
+ * are incomplete (TLAG_ESTATE).  tlag_seed, tlag_step, tlag_run, tlag_restart and tlag_destroy release the graph; reading
+ * a released graph is TLAG_ESTATE.  device_ms: from the index pass to the last append (CUDA events). */
+typedef struct {
+  uint64_t n_states, n_expanded, n_edges;
+  float    device_ms;
+} tlag_graph_info;
+
+int  tlag_build_graph(tlag_engine *e, tlag_graph_info *out);
+/* The edges of rows [first, first + n): off_out n + 1 offsets relative to row `first` (off_out[0] = 0), dst_out and
+ * act_out off_out[n] destination rows and action ids.  dst_out / act_out may be NULL (sizing). */
+int  tlag_read_graph(tlag_engine *e, uint64_t first, uint64_t n, uint64_t *off_out, uint32_t *dst_out, int32_t *act_out);
+/* XOR and SUM (mod 2^64) over all edges (s, t, a) of the edge term of csrc/tlag_vm.h (tlag_edge_term) on the
+ * fingerprints of s and t and on a: does not depend on the store's order. */
+int  tlag_graph_digest(tlag_engine *e, uint64_t *xor_out, uint64_t *sum_out);
+
 /* ---- multi-GPU building blocks (one engine per rank; the host exchanges the buffers,
  *      e.g. torch.distributed all_to_all_single over NCCL/NVLink; SURVEY.md §8e) ---------- */
 /* Expand the current frontier WITHOUT inserting: successor records (W state words + parent

@@ -48,12 +48,14 @@ def pcal2tla_main(argv=None):
 
 
 def check_file(path, deadlock=True, cfg_path=None, out=None, device=0, seq_cap=None, verbose=True, lib_dirs=(),
-               engine="auto", max_depth=0, simulate=None):
+               engine="auto", max_depth=0, simulate=None, dump=None):
     """engine: "interp" = bytecode interpreter kernel, "sliced" = the model compiled to one CUDA kernel per slice of its
     program (nvcc at run time, cached in csrc/native/), "auto" = sliced for programs big enough to repay the compile.
     max_depth = L: stop after level L exists (levels 1..L-1 expanded) and report the prefix.
     simulate = (num, seed): random simulation instead of the search, num behaviours of at most max_depth states (100 when
-    0) from the given seed (include/tlag.h: tlag_simulate)."""
+    0) from the given seed (include/tlag.h: tlag_simulate).
+    dump = (path, dot qualifiers or None): after the report, write every stored state to path (TLC's -dump), or with
+    qualifiers the state graph in Graphviz form (TLC's -dump dot)."""
     from .checker import compile_model, encode_states, result_from_engine
     from .engine import Engine
     t0 = time.time()
@@ -121,6 +123,7 @@ def check_file(path, deadlock=True, cfg_path=None, out=None, device=0, seq_cap=N
             e = Engine(cm, deadlock=deadlock and m.check_deadlock, device=device, native=native)
             e.seed(iw)
             r0 = e.result()
+            levels = [r0["distinct"]]            # states per BFS level, in store order (the order -dump numbers them in)
             print(f"Finished computing initial states: {r0['distinct']} distinct state"
                   f"{'s' if r0['distinct'] != 1 else ''} generated.", file=out)
             while True:
@@ -128,6 +131,8 @@ def check_file(path, deadlock=True, cfg_path=None, out=None, device=0, seq_cap=N
                     print(f"Depth bound {max_depth} reached: the states of the last level were not expanded.", file=out)
                     break
                 ws = e.step()
+                if ws.get("discovered"):
+                    levels.append(ws["discovered"])
                 if ws["verdict"] != 5:
                     break
                 if verbose and ws["expanded"]:
@@ -148,6 +153,7 @@ def check_file(path, deadlock=True, cfg_path=None, out=None, device=0, seq_cap=N
         _types.SPARSE_CAP = base_sparse
     if simulate is not None:
         return _report_simulation(path, m, cm, r, e, simulate[1], t0, out)
+    dumped = _dump(e, cm, m, levels, *dump) if dump is not None else None
     if int(os.environ.get("WORLD_SIZE", "1")) == 1:
         # The parallel search reports an error with the counts of the whole level it was found in, and with whichever of
         # several shortest behaviours won the race.  TLC's single worker stops AT the first Assert failure / deadlock
@@ -167,10 +173,55 @@ def check_file(path, deadlock=True, cfg_path=None, out=None, device=0, seq_cap=N
     text = format_result(res, m.vars, m.module_name)
     print(text, file=out)
     _write_reports(path, m, res, text)
+    if dumped is not None:
+        print(dumped(), file=out)
     print(f"Finished in {time.time() - t0:.2f}s ({r['device_seconds']:.4f}s in GPU wave kernels, "
           f"{e.launches()} kernel launches).", file=out)
     e.close()
     return 0 if res.verdict == OK else 12
+
+
+def _dump(e, cm, m, levels, path, dot):
+    """`tlc -dump`: reads what the dump needs from the search's engine now (before an exact replay closes it) and returns
+    the function that writes it (after the report) and says so.  States are numbered from 1 by BFS level, then by
+    ascending 64-bit fingerprint within a level; with `dot` (the qualifiers) the nodes are those numbers, initial states
+    filled, and the edges come from the state graph the engine builds in device memory."""
+    from .checker import decode_state
+    from .engine import EngineError
+    from .fingerprint import fingerprint_words
+    from .front.report import format_state
+    n = sum(levels)
+    words = e.read_states(0, n) if n else []
+    order, a = [], 0
+    for size in levels:
+        order += sorted(range(a, a + size), key=lambda i: fingerprint_words(words[i]))
+        a += size
+    num = {row: k for k, row in enumerate(order, 1)}
+    text = {row: format_state(decode_state(cm, words[row]), m.vars) for row in order}
+    edges = None
+    if dot is not None:
+        try:
+            e.build_graph()
+            off, dst, act = e.state_graph(0, n)
+        except EngineError as ex:
+            return lambda: f"The state graph was not dumped: {ex}"
+        edges = sorted((num[s], num[int(dst[j])], int(act[j])) for s in range(n) for j in range(int(off[s]), int(off[s + 1])))
+
+    def write():
+        with open(path, "w") as f:
+            if edges is None:
+                for row in order:
+                    f.write(f"State {num[row]}:\n{text[row]}\n\n")
+                return f"Dumped {n} states to {path}."
+            f.write("digraph StateGraph {\n")
+            for row in order:
+                label = text[row].replace("\\", "\\\\").replace('"', '\\"').replace("\n", "\\n")
+                f.write(f'{num[row]} [label="{label}"{",style=filled" if row < levels[0] else ""}];\n')
+            for k, j, a_ in edges:
+                f.write(f'{k} -> {j} [label="{cm.actions[a_][0]}"];\n')
+            f.write("}\n")
+        return f"Dumped the state graph ({n} states, {len(edges)} transitions) to {path}."
+    return write
 
 
 def _write_reports(path, m, res, text):
@@ -263,7 +314,7 @@ def _free_port():
 def tlc_main(argv=None):
     argv = list(sys.argv[1:] if argv is None else argv)
     files, deadlock, cfg, dev, libs, seq_cap, engine, depth, gpus = [], True, None, 0, [], None, "auto", 0, 1
-    sim_num, seed = None, None
+    sim_num, seed, dump = None, None, None
     i = 0
     while i < len(argv):
         a = argv[i]
@@ -292,6 +343,17 @@ def tlc_main(argv=None):
         elif a == "-seed":
             i += 1
             seed = int(argv[i])
+        elif a == "-dump":                  # -dump FILE: the states; -dump dot[,qualifiers] FILE: the state graph
+            i += 1
+            if argv[i] == "dot" or argv[i].startswith("dot,"):
+                dump = (argv[i + 1], argv[i].split(",")[1:])
+                # TLC's qualifiers are accepted so that its command lines work; the edges always carry their action
+                for q in dump[1]:
+                    if q not in ("actionlabels", "colorize", "snapshot"):
+                        print(f"Warning: -dump dot: unknown qualifier {q} ignored.")
+                i += 1
+            else:
+                dump = (argv[i], None)
         elif a == "-gpus":                  # partition the state space over N GPUs of this box (one process per GPU)
             i += 1
             gpus = int(argv[i])
@@ -306,7 +368,10 @@ def tlc_main(argv=None):
         i += 1
     if not files:
         print("usage: tlc [-deadlock] [-config FILE.cfg] [-I DIR] [-seqcap N] [-engine interp|sliced|auto] [-depth N] [-gpus N] "
-              "[-simulate [num=K] [-seed S]] FILE.tla ...", file=sys.stderr)
+              "[-simulate [num=K] [-seed S]] [-dump [dot[,...]] FILE] FILE.tla ...", file=sys.stderr)
+        return 2
+    if dump is not None and (sim_num is not None or gpus > 1):
+        print("tlc: -dump writes the states of a search on one GPU: drop -simulate and -gpus", file=sys.stderr)
         return 2
     if sim_num is not None and gpus > 1:
         print("tlc: -simulate runs on one GPU: drop -gpus", file=sys.stderr)
@@ -348,7 +413,8 @@ def tlc_main(argv=None):
             print(f"Running random simulation with seed {seed}.")
         try:
             r = check_file(f, deadlock=deadlock, cfg_path=cfg, device=dev, lib_dirs=libs, seq_cap=seq_cap,
-                           engine=engine, max_depth=depth, simulate=None if sim_num is None else (sim_num, seed))
+                           engine=engine, max_depth=depth, simulate=None if sim_num is None else (sim_num, seed),
+                           dump=dump)
         except (SpecError, ParseError, LexError, EvalError, CompileError, TypeErr) as ex:
             print(f"Error: {type(ex).__name__}: {ex}")
             r = 150

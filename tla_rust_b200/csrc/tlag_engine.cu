@@ -22,6 +22,7 @@
 #include <unordered_set>
 #include <vector>
 #include <cub/device/device_radix_sort.cuh>   // CUDA-toolkit header library; used only to reorder a level (not on the hot path)
+#include <cub/device/device_select.cuh>       // (and by the state graph pass: duplicate edges of a chunk)
 
 #include "tlag_dev.cuh"
 // second copy of the instruction executor without the extension ops (see tlag_vm_exec.inc)
@@ -104,6 +105,10 @@ struct tlag_engine {
   uint32_t* d_hist = nullptr; int16_t* d_act = nullptr; uint8_t* d_sstat = nullptr; uint8_t* d_ssucc = nullptr;
   uint32_t* d_scnt = nullptr; uint32_t* d_slen = nullptr; SimCtl* d_sctl = nullptr; uint32_t* d_sinit = nullptr;
   uint64_t sim_B = 0, sim_D = 0, sim_n = 0, sim_first = 0, sim_n_init = 0;
+  // state graph (tlag_build_graph): CSR over the store's rows, offsets g_states + 1, released when the search moves on
+  unsigned long long* d_goff = nullptr; uint32_t* d_gdst = nullptr; uint32_t* d_gact = nullptr;
+  uint64_t g_cap = 0, g_edges = 0, g_states = 0, g_expanded = 0; bool g_ready = false;
+  uint64_t graph_edges = 1ULL << 24;  // edges the chunk buffer of the edge pass starts with (TLAG_GRAPH_EDGES: test hook)
 };
 
 // ------------------------------------------------------------------ sliced native build
@@ -147,7 +152,6 @@ __global__ void k_sl_deadlock(DevParams p, unsigned long long lo, unsigned long 
 }
 #endif  // TLAG_SLICED_INC
 
-#ifndef TLAG_SLICED_INC
 // ------------------------------------------------------------------ wave kernel
 // Warp-scheduled interpreter.  A SIMT interpreter that lets every lane follow its own pc pays a
 // divergent fetch/decode/dispatch per distinct opcode per step.  Here the warp executes, at every
@@ -177,6 +181,8 @@ __device__ __forceinline__ void warp_vm(const uint64_t* __restrict__ gcode, cons
     }
   }
 }
+
+#ifndef TLAG_SLICED_INC   // (a sliced library runs the interpreter only in the state graph's edge pass, k_graph)
 
 // MODE 0: fused insert (single GPU).  MODE 1: route successors to per-owner send regions.
 // LEAN: interpreter without the extension ops, for models that do not use them (small frames only).
@@ -434,6 +440,173 @@ __global__ void k_sim_digest(SimParams s, int W, unsigned long long n, unsigned 
   for (int o = 16; o > 0; o >>= 1) { x ^= __shfl_down_sync(0xffffffffu, x, o); sm += __shfl_down_sync(0xffffffffu, sm, o); }
   if ((threadIdx.x & 31) == 0) { atomicXor(&out2[0], x); atomicAdd(&out2[1], sm); }
 }
+
+#if !defined(TLAG_SL_SIM)
+// ------------------------------------------------------------------ state graph (tlag_build_graph), both engines
+// The index pass maps each seen-set slot to the store row whose fingerprint it holds; the edge pass runs Next on a chunk
+// of expanded rows with the interpreter and finds each successor's row by a read-only probe of the same seen-set.
+struct GraphCtl {
+  unsigned long long n;             // edges the chunk produced (counted past the buffer's capacity)
+  unsigned long long missing;       // a fingerprint without a slot, or a successor that is not stored
+  unsigned long long bad;           // the edge pass met an evaluation trap, a pack overflow or an action id out of range
+};
+
+struct GraphParams {
+  const uint32_t* row_of_slot;      // seen-set slot -> store row
+  unsigned long long first;         // first row of the chunk
+  unsigned long long* keys;         // the chunk's edges: (s - first) << (32 + abits) | t << abits | a
+  unsigned long long cap;
+  unsigned abits;
+  GraphCtl* ctl;
+};
+
+// the slot of fp in the seen-set, or -1 when it is not there (read-only: the probe sequence of seen_insert)
+__device__ __forceinline__ long long seen_find(const unsigned long long* __restrict__ table, unsigned long long mask,
+                                               unsigned long long fp) {
+  unsigned long long i = fp & mask;
+  for (unsigned long long probes = 0; probes <= mask; ++probes, i = (i + 1) & mask) {
+    const unsigned long long v = table[i];
+    if (v == fp) return (long long)i;
+    if (v == 0ULL) return -1;
+  }
+  return -1;
+}
+
+__global__ void k_graph_index(DevParams p, unsigned long long n, uint32_t* __restrict__ row_of_slot, GraphCtl* ctl) {
+  const unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  uint32_t w[TLAG_MAXW];
+  for (int k = 0; k < p.W; ++k) w[k] = p.states[i * (unsigned long long)p.W + k];
+  const long long slot = seen_find(p.table, p.mask, tlag_fingerprint(w, p.W));
+  if (slot < 0) atomicExch(&ctl->missing, 1ULL);
+  else row_of_slot[slot] = (uint32_t)i;
+}
+
+// Edges out of rows [g.first, hi): one lane per row, the warp-scheduled interpreter of k_wave on Next only (no invariant,
+// nothing reported to the search's counters).  Each EMIT is packed, fingerprinted and looked up; a successor other than
+// the row itself is appended to the chunk's buffer, one atomic per warp.
+template <int FRAME, bool SMEM, bool LEAN>
+__global__ void __launch_bounds__(TLAG_BLOCK, TLAG_WAVE_OCC(FRAME, SMEM))
+k_graph(DevParams p, GraphParams g, unsigned long long hi) {
+  extern __shared__ uint64_t s_code[];
+  if (SMEM) {
+    for (uint32_t i = threadIdx.x; i < p.code_len; i += blockDim.x) s_code[i] = p.code[i];
+    __syncthreads();
+  }
+  const uint64_t* code = p.code;
+  int32_t frame[FRAME];
+  uint32_t succ[TLAG_MAXW];
+  const unsigned lane = threadIdx.x & 31;
+  const int W = p.W;
+  const unsigned long long stride = (unsigned long long)gridDim.x * blockDim.x;
+  for (unsigned long long base = g.first + (unsigned long long)blockIdx.x * blockDim.x + (threadIdx.x & ~31u); base < hi;
+       base += stride) {
+    const unsigned long long idx = base + lane;
+    const bool active = idx < hi;
+    if (active) {
+      const uint32_t* src = p.states + idx * (unsigned long long)W;
+      for (int i = 0; i < W; ++i) succ[i] = src[i];
+      tlag_unpack(p.layout, p.n_slots, succ, frame + p.n_off);
+    }
+    int st = active ? L_RUN : L_DONE, ev = 0;
+    int32_t info = 0, info2 = 0;
+    uint32_t pc = active ? p.entry_next : TLAG_PC_PARKED, rpc = 0;
+    for (;;) {
+      warp_vm<SMEM, LEAN>(code, s_code, p.cpool, frame, pc, rpc, ev, info, info2);
+      if (st == L_RUN) {
+        if (ev == TLAG_EV_EMIT) st = L_EMIT;
+        else if (ev == TLAG_EV_HALT) st = L_DONE;
+        else if (ev == TLAG_EV_GEN || ev == TLAG_EV_INVF || ev == TLAG_EV_ASSERT) pc = rpc;
+        else { atomicExch(&g.ctl->bad, 1ULL); st = L_DONE; }
+      }
+      if (__any_sync(0xffffffffu, pc != TLAG_PC_PARKED)) continue;
+      if (!__any_sync(0xffffffffu, st == L_EMIT)) break;
+      bool keep = false;
+      unsigned long long key = 0;
+      if (st == L_EMIT) {
+        int ov;
+        if (!LEAN && info2 > 0) {
+          const uint32_t* src = p.states + idx * (unsigned long long)W;
+          for (int i = 0; i < W; ++i) succ[i] = src[i];
+          ov = tlag_pack_ranges(p.layout, p.cpool, info2, frame + p.p_off, succ);
+        } else {
+          ov = tlag_pack(p.layout, p.n_slots, frame + p.p_off, succ, W);
+        }
+        if (ov || info < 0 || ((unsigned long long)info >> g.abits) != 0) {
+          atomicExch(&g.ctl->bad, 1ULL);
+        } else {
+          const long long slot = seen_find(p.table, p.mask, tlag_fingerprint(succ, W));
+          if (slot < 0) {
+            atomicExch(&g.ctl->missing, 1ULL);
+          } else {
+            const unsigned long long t = g.row_of_slot[slot];
+            keep = t != idx;
+            key = ((idx - g.first) << (32 + g.abits)) | (t << g.abits) | (unsigned long long)info;
+          }
+        }
+        st = L_RUN; pc = rpc;
+      }
+      const unsigned m = __ballot_sync(0xffffffffu, keep);
+      if (keep) {
+        const int leader = __ffs((int)m) - 1;
+        unsigned long long pos = 0;
+        if ((int)lane == leader) pos = atomicAdd(&g.ctl->n, (unsigned long long)__popc(m));
+        pos = __shfl_sync(m, pos, leader) + (unsigned long long)__popc(m & lanemask_lt());
+        if (pos < g.cap) g.keys[pos] = key;
+      }
+    }
+  }
+}
+
+// Rows [0, rows] of a chunk whose sorted distinct edges are keys[0, n): off[r] = base + the first edge of row r
+__global__ void k_graph_rows(const unsigned long long* __restrict__ keys, unsigned long long n, unsigned long long rows,
+                             unsigned shift, unsigned long long base, unsigned long long* __restrict__ off) {
+  const unsigned long long r = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (r > rows) return;
+  unsigned long long lo = 0, hi = n;
+  while (lo < hi) {
+    const unsigned long long mid = (lo + hi) >> 1;
+    if ((keys[mid] >> shift) < r) lo = mid + 1; else hi = mid;
+  }
+  off[r] = base + lo;
+}
+
+// edge i of the chunk -> its destination row and action id in the resident CSR
+__global__ void k_graph_split(const unsigned long long* __restrict__ keys, unsigned long long n, unsigned abits,
+                              uint32_t* __restrict__ dst, uint32_t* __restrict__ act) {
+  const unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const unsigned long long k = keys[i];
+  dst[i] = (uint32_t)(k >> abits);
+  act[i] = (uint32_t)(k & ((1ULL << abits) - 1));
+}
+
+__global__ void k_fill_u64(unsigned long long* __restrict__ a, unsigned long long n, unsigned long long v) {
+  const unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) a[i] = v;
+}
+
+// XOR and SUM of tlag_edge_term over the edges out of rows [0, n)
+__global__ void k_graph_digest(DevParams p, const unsigned long long* __restrict__ off, const uint32_t* __restrict__ dst,
+                               const uint32_t* __restrict__ act, unsigned long long n, unsigned long long* out2) {
+  unsigned long long x = 0, sm = 0;
+  uint32_t w[TLAG_MAXW];
+  for (unsigned long long s = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; s < n;
+       s += (unsigned long long)gridDim.x * blockDim.x) {
+    if (off[s] == off[s + 1]) continue;
+    for (int k = 0; k < p.W; ++k) w[k] = p.states[s * (unsigned long long)p.W + k];
+    const unsigned long long fs = tlag_fingerprint(w, p.W);
+    for (unsigned long long j = off[s]; j < off[s + 1]; ++j) {
+      const unsigned long long t = dst[j];
+      for (int k = 0; k < p.W; ++k) w[k] = p.states[t * (unsigned long long)p.W + k];
+      const unsigned long long v = tlag_edge_term(fs, tlag_fingerprint(w, p.W), (int32_t)act[j]);
+      x ^= v; sm += v;
+    }
+  }
+  for (int o = 16; o > 0; o >>= 1) { x ^= __shfl_down_sync(0xffffffffu, x, o); sm += __shfl_down_sync(0xffffffffu, sm, o); }
+  if ((threadIdx.x & 31) == 0) { atomicXor(&out2[0], x); atomicAdd(&out2[1], sm); }
+}
+#endif  // !TLAG_SL_SIM
 
 // ------------------------------------------------------------------ K1 alone: fingerprint + probe/insert
 // One thread per candidate state, word by word: the inputs the staged form does not take (W = 1, or a batch that is not
@@ -1228,6 +1401,18 @@ static void read_env_hooks(tlag_engine* e) {
     while (e->rset_log2 < 40 && (1L << e->rset_log2) < n) ++e->rset_log2;
     e->rset_fixed = true;
   }
+  // n starts the state graph's edge buffer at n edges (tlag_build_graph), so that chunks overflow it and are run again
+  // with fewer rows
+  s_ = getenv("TLAG_GRAPH_EDGES");
+  if (s_ && *s_ && atoll(s_) > 0) e->graph_edges = (uint64_t)atoll(s_);
+}
+
+// The state graph is a picture of the store after a search call: any call that changes the store drops it.
+static void release_graph(tlag_engine* e) {
+  dfree(e, e->d_goff); dfree(e, e->d_gdst); dfree(e, e->d_gact);
+  e->d_goff = nullptr; e->d_gdst = e->d_gact = nullptr;
+  e->g_cap = e->g_edges = e->g_states = e->g_expanded = 0;
+  e->g_ready = false;
 }
 
 extern "C" int tlag_create(const tlag_model* m, tlag_engine** out) {
@@ -1325,6 +1510,7 @@ extern "C" void tlag_destroy(tlag_engine* e) {
     dfree(e, e->d_scratch); dfree(e, e->d_flags); dfree(e, e->d_disc); dfree(e, e->d_sort); dfree(e, e->d_rset); dfree(e, e->d_sent); dfree(e, e->d_succ);
     dfree(e, e->d_hist); dfree(e, e->d_act); dfree(e, e->d_sstat); dfree(e, e->d_ssucc); dfree(e, e->d_scnt); dfree(e, e->d_slen);
     dfree(e, e->d_sinit);
+    release_graph(e);
     cudaStreamSynchronize(e->stream);
   }
   if (e->p2p_slot >= 0) {                              // exchange buffers and peer mappings are parked, not released
@@ -1403,6 +1589,7 @@ extern "C" int tlag_reset_table(tlag_engine* e) {
 extern "C" int tlag_seed(tlag_engine* e, const uint32_t* states, uint64_t n) {
   if (!e || (!states && n)) return TLAG_EINVAL;
   if (e->level != 0) { e->err = "tlag_seed after the search started"; return TLAG_ESTATE; }
+  release_graph(e);
   const uint64_t W = e->m.words_per_state;
   int r = reserve_level(e, e->hi + n + 1024, e->hi + n);
   if (r) return r;
@@ -1441,6 +1628,7 @@ extern "C" int tlag_seed(tlag_engine* e, const uint32_t* states, uint64_t n) {
 // Forget everything discovered and start again from the retained initial states (bench loops).
 extern "C" int tlag_restart(tlag_engine* e) {
   if (!e) return TLAG_EINVAL;
+  release_graph(e);
   end_appends(e);
   CK(reset_counters(e, 0));
   CK(cudaMemsetAsync(e->d_table, 0, (1ULL << e->table_log2) * 8, e->stream));
@@ -1583,6 +1771,7 @@ extern "C" int tlag_step(tlag_engine* e, tlag_wave_stats* out) {
   TLAG_NO_BFS(e);
 #endif
   if (out) memset(out, 0, sizeof(*out));
+  release_graph(e);
   start_search(e);
   if (e->verdict != TLAG_V_RUNNING) { if (out) out->verdict = e->verdict; return TLAG_OK; }
   const uint64_t lo = e->lo, hi = e->hi;
@@ -2216,6 +2405,314 @@ extern "C" int tlag_sim_digest(tlag_engine* e, uint64_t* xor_out, uint64_t* sum_
   k_sim_digest<<<e->sm_count * 8, 256, 0, e->stream>>>(s, (int)e->m.words_per_state, e->sim_n, e->d_dig);
   e->launches++;
   CK(cudaGetLastError());
+  unsigned long long h2[2];
+  CK(cudaMemcpyAsync(h2, e->d_dig, 16, cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaStreamSynchronize(e->stream));
+  *xor_out = h2[0]; *sum_out = h2[1];
+  return TLAG_OK;
+#endif
+}
+
+// ---- state graph (include/tlag.h: tlag_build_graph) -------------------------------------------------------------------
+#if !defined(TLAG_SL_SIM)
+#if defined(TLAG_SLICED_INC)
+// a sliced library holds one variant of the edge pass: the frame class of its model and, as tlag_create decides for the
+// interpreter, the program in shared memory when it fits
+#if TLAG_SL_FRAME <= 64
+#define TLAG_GRAPH_FRAME 64
+#elif TLAG_SL_FRAME <= 128
+#define TLAG_GRAPH_FRAME 128
+#elif TLAG_SL_FRAME <= 256
+#define TLAG_GRAPH_FRAME 256
+#elif TLAG_SL_FRAME <= 512
+#define TLAG_GRAPH_FRAME 512
+#elif TLAG_SL_FRAME <= 1024
+#define TLAG_GRAPH_FRAME 1024
+#elif TLAG_SL_FRAME <= 2048
+#define TLAG_GRAPH_FRAME 2048
+#elif TLAG_SL_FRAME <= 4096
+#define TLAG_GRAPH_FRAME 4096
+#else
+#define TLAG_GRAPH_FRAME 8192
+#endif
+#define TLAG_GRAPH_SMEM (TLAG_SL_FRAME <= 512 && TLAG_NATIVE_CODE_LEN * 8ull <= 200ull * 1024)
+#endif
+
+static cudaError_t launch_graph(tlag_engine* e, const GraphParams& g, uint64_t hi) {
+  void (*fn)(DevParams, GraphParams, unsigned long long) = nullptr;
+#if defined(TLAG_SLICED_INC)
+  const bool sm = TLAG_GRAPH_SMEM;
+  fn = k_graph<TLAG_GRAPH_FRAME, TLAG_GRAPH_SMEM, false>;
+#else
+  const bool sm = e->p.code_in_smem != 0;
+  const bool lean = !e->uses_ext;
+  switch (e->frame_class) {
+    case 0: fn = lean ? (sm ? k_graph<64, true, true> : k_graph<64, false, true>) : (sm ? k_graph<64, true, false> : k_graph<64, false, false>); break;
+    case 1: fn = lean ? (sm ? k_graph<128, true, true> : k_graph<128, false, true>) : (sm ? k_graph<128, true, false> : k_graph<128, false, false>); break;
+    case 2: fn = lean ? (sm ? k_graph<256, true, true> : k_graph<256, false, true>) : (sm ? k_graph<256, true, false> : k_graph<256, false, false>); break;
+    case 3: fn = lean ? (sm ? k_graph<512, true, true> : k_graph<512, false, true>) : (sm ? k_graph<512, true, false> : k_graph<512, false, false>); break;
+    case 4: fn = sm ? k_graph<1024, true, false> : k_graph<1024, false, false>; break;
+    case 5: fn = sm ? k_graph<2048, true, false> : k_graph<2048, false, false>; break;
+    case 6: fn = sm ? k_graph<4096, true, false> : k_graph<4096, false, false>; break;
+    default: fn = sm ? k_graph<8192, true, false> : k_graph<8192, false, false>; break;
+  }
+#endif
+  const size_t smem = sm ? (size_t)e->p.code_len * 8 : 0;
+  if (smem > 48 * 1024) {
+    cudaError_t r = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (r != cudaSuccess) return r;
+  }
+  int occ = 1;
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, fn, TLAG_BLOCK, smem) != cudaSuccess || occ < 1) occ = 1;
+  uint64_t blocks = (hi - g.first + TLAG_BLOCK - 1) / TLAG_BLOCK;
+  if (blocks > (uint64_t)e->sm_count * (uint64_t)occ) blocks = (uint64_t)e->sm_count * (uint64_t)occ;
+  if (blocks == 0) blocks = 1;
+  fn<<<(unsigned)blocks, TLAG_BLOCK, smem, e->stream>>>(e->p, g, hi);
+  e->launches++;
+  return cudaGetLastError();
+}
+
+static unsigned bits_for(uint64_t n) {   // bits of n - 1, at least 1
+  unsigned b = 1;
+  while (b < 64 && (1ULL << b) < n) ++b;
+  return b;
+}
+
+// The resident CSR holds at least `need` edges (geometric growth up to `bound`, contents kept)
+static int graph_reserve(tlag_engine* e, uint64_t need, uint64_t bound) {
+  if (need <= e->g_cap) return TLAG_OK;
+  uint64_t cap = e->g_cap * 2 > need ? e->g_cap * 2 : need;
+  if (cap > bound && bound >= need) cap = bound;
+  uint32_t *nd = nullptr, *na = nullptr;
+  if (dmalloc(e, &nd, cap * 4) != cudaSuccess || dmalloc(e, &na, cap * 4) != cudaSuccess) {
+    cudaGetLastError();
+    dfree(e, nd); dfree(e, na);
+    e->err = "tlag_build_graph: not enough device memory for the state graph";
+    return TLAG_ENOMEM;
+  }
+  if (e->g_edges) {
+    CK(cudaMemcpyAsync(nd, e->d_gdst, e->g_edges * 4, cudaMemcpyDeviceToDevice, e->stream));
+    CK(cudaMemcpyAsync(na, e->d_gact, e->g_edges * 4, cudaMemcpyDeviceToDevice, e->stream));
+  }
+  dfree(e, e->d_gdst); dfree(e, e->d_gact);
+  e->d_gdst = nd; e->d_gact = na; e->g_cap = cap;
+  return TLAG_OK;
+}
+
+// The passes of tlag_build_graph over n_states stored rows, n_exp of them expanded; scratch buffers freed by the caller
+struct GraphScratch { uint32_t* row_of_slot = nullptr; unsigned long long* keys = nullptr; void* tmp = nullptr; GraphCtl* ctl = nullptr; };
+
+static int graph_passes(tlag_engine* e, GraphScratch& sc, uint64_t n_states, uint64_t n_exp) {
+  const uint64_t slots = e->p.mask + 1;
+  const unsigned abits = bits_for(e->m.n_actions ? e->m.n_actions : 1);
+  if (abits > 24) { e->err = "tlag_build_graph: more than 2^24 actions"; return TLAG_EINVAL; }
+  const uint64_t max_rows = 1ULL << (32 - abits);         // (s - first) | t | a fit one 64-bit key
+  uint64_t cap = e->graph_edges;
+  size_t sort_tmp = 0, uniq_tmp = 0;
+  {
+    cub::DoubleBuffer<unsigned long long> k(nullptr, nullptr);
+    cub::DeviceRadixSort::SortKeys(nullptr, sort_tmp, k, (unsigned long long)cap);
+    cub::DeviceSelect::Unique(nullptr, uniq_tmp, (unsigned long long*)nullptr, (unsigned long long*)nullptr,
+                              (unsigned long long*)nullptr, (unsigned long long)cap);
+  }
+  size_t tmp_bytes = ((sort_tmp > uniq_tmp ? sort_tmp : uniq_tmp) + 255) & ~(size_t)255;   // then the count of Unique
+  if (dmalloc(e, &sc.row_of_slot, slots * 4) != cudaSuccess || dmalloc(e, &sc.keys, cap * 16) != cudaSuccess ||
+      dmalloc(e, &sc.tmp, tmp_bytes + 256) != cudaSuccess || dmalloc(e, &sc.ctl, sizeof(GraphCtl)) != cudaSuccess) {
+    cudaGetLastError();
+    e->err = "tlag_build_graph: not enough device memory for the index and edge buffers";
+    return TLAG_ENOMEM;
+  }
+  if (dmalloc(e, &e->d_goff, (n_states + 1) * 8) != cudaSuccess) {
+    cudaGetLastError();
+    e->err = "tlag_build_graph: not enough device memory for the state graph";
+    return TLAG_ENOMEM;
+  }
+  e->g_states = n_states; e->g_expanded = n_exp;
+  // every edge was an EMIT the search counted in `generated`: reserve that many at once (no copy of a multi-GB CSR
+  // while it grows), and grow from 2^20 edges when it does not fit
+  const uint64_t init_gen = e->h_init.size() / e->m.words_per_state;
+  const uint64_t bound = e->generated > init_gen ? e->generated - init_gen : 0;
+  int r = graph_reserve(e, bound ? bound : 1, bound);
+  if (r == TLAG_ENOMEM) r = graph_reserve(e, (1ULL << 20) < bound ? (1ULL << 20) : (bound ? bound : 1), bound);
+  if (r) return r;
+
+  // index pass: row_of_slot[slot of row i's fingerprint] = i
+  CK(cudaMemsetAsync(sc.ctl, 0, sizeof(GraphCtl), e->stream));
+  if (n_states) {
+    k_graph_index<<<(unsigned)((n_states + 255) / 256), 256, 0, e->stream>>>(e->p, n_states, sc.row_of_slot, sc.ctl);
+    e->launches++;
+    CK(cudaGetLastError());
+  }
+  // chunks of expanded rows, sized from the search's successors per expanded state; a chunk whose edges overflow the
+  // buffer is run again with half the rows (a single row: with a buffer as big as its count)
+  const double ratio = n_exp ? (double)bound / (double)n_exp : 1.0;
+  uint64_t rows = (uint64_t)((double)cap / (ratio + 1.0));
+  GraphCtl hc;
+  for (uint64_t first = 0; first < n_exp;) {
+    if (rows < 1) rows = 1;
+    if (rows > max_rows) rows = max_rows;
+    const uint64_t n = n_exp - first < rows ? n_exp - first : rows;
+    GraphParams g;
+    g.row_of_slot = sc.row_of_slot; g.first = first; g.keys = sc.keys; g.cap = cap; g.abits = abits; g.ctl = sc.ctl;
+    CK(cudaMemsetAsync(&sc.ctl->n, 0, 8, e->stream));
+    CK(launch_graph(e, g, first + n));
+    CK(cudaMemcpyAsync(&hc, sc.ctl, sizeof(hc), cudaMemcpyDeviceToHost, e->stream));
+    CK(cudaStreamSynchronize(e->stream));
+    if (hc.missing) {
+      e->err = "tlag_build_graph: a stored state or a successor of an expanded state is not in the seen-set (store and "
+               "seen-set disagree)";
+      return TLAG_ESTATE;
+    }
+    if (hc.bad) { e->err = "tlag_build_graph: Next trapped while its successors were enumerated again"; return TLAG_ESTATE; }
+    if (hc.n > cap) {
+      if (n > 1) { rows = n / 2; continue; }
+      dfree(e, sc.keys); dfree(e, sc.tmp); sc.keys = nullptr; sc.tmp = nullptr;
+      cap = hc.n;
+      cub::DoubleBuffer<unsigned long long> k(nullptr, nullptr);
+      cub::DeviceRadixSort::SortKeys(nullptr, sort_tmp, k, (unsigned long long)cap);
+      cub::DeviceSelect::Unique(nullptr, uniq_tmp, (unsigned long long*)nullptr, (unsigned long long*)nullptr,
+                                (unsigned long long*)nullptr, (unsigned long long)cap);
+      tmp_bytes = ((sort_tmp > uniq_tmp ? sort_tmp : uniq_tmp) + 255) & ~(size_t)255;
+      if (dmalloc(e, &sc.keys, cap * 16) != cudaSuccess || dmalloc(e, &sc.tmp, tmp_bytes + 256) != cudaSuccess) {
+        cudaGetLastError();
+        e->err = "tlag_build_graph: not enough device memory for the edges of one state";
+        return TLAG_ENOMEM;
+      }
+      continue;
+    }
+    // sort by (s, t, a), drop duplicates, append to the CSR
+    const uint64_t m = hc.n;
+    unsigned long long* ka = sc.keys; unsigned long long* kb = sc.keys + cap;
+    unsigned long long* d_nsel = (unsigned long long*)((uint8_t*)sc.tmp + tmp_bytes);
+    uint64_t nu = 0;
+    if (m) {
+      cub::DoubleBuffer<unsigned long long> k(ka, kb);
+      size_t tb = tmp_bytes;
+      if (cub::DeviceRadixSort::SortKeys(sc.tmp, tb, k, (unsigned long long)m, 0, (int)(32 + abits + bits_for(n)),
+                                         e->stream) != cudaSuccess) { e->err = "cub sort failed"; return TLAG_ECUDA; }
+      unsigned long long* sorted = k.Current();
+      unsigned long long* uniq = sorted == ka ? kb : ka;
+      tb = tmp_bytes;
+      if (cub::DeviceSelect::Unique(sc.tmp, tb, sorted, uniq, d_nsel, (unsigned long long)m, e->stream) != cudaSuccess) {
+        e->err = "cub unique failed"; return TLAG_ECUDA;
+      }
+      e->launches += 2;
+      CK(cudaMemcpyAsync(&nu, d_nsel, 8, cudaMemcpyDeviceToHost, e->stream));
+      CK(cudaStreamSynchronize(e->stream));
+      r = graph_reserve(e, e->g_edges + nu, bound);
+      if (r) return r;
+      k_graph_split<<<(unsigned)((nu + 255) / 256), 256, 0, e->stream>>>(
+          uniq, nu, abits, e->d_gdst + e->g_edges, e->d_gact + e->g_edges);
+      k_graph_rows<<<(unsigned)((n + 1 + 255) / 256), 256, 0, e->stream>>>(uniq, nu, n, 32 + abits, e->g_edges,
+                                                                          e->d_goff + first);
+      e->launches += 2;
+    } else {
+      k_fill_u64<<<(unsigned)((n + 1 + 255) / 256), 256, 0, e->stream>>>(e->d_goff + first, n + 1, e->g_edges);
+      e->launches++;
+    }
+    CK(cudaGetLastError());
+    e->g_edges += nu;
+    first += n;
+  }
+  // rows past the expanded ones have no edges
+  k_fill_u64<<<(unsigned)((n_states - n_exp + 1 + 255) / 256), 256, 0, e->stream>>>(e->d_goff + n_exp, n_states - n_exp + 1,
+                                                                                     e->g_edges);
+  e->launches++;
+  CK(cudaGetLastError());
+  CK(cudaMemcpyAsync(&hc, sc.ctl, sizeof(hc), cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaStreamSynchronize(e->stream));
+  if (hc.missing) { e->err = "tlag_build_graph: a stored state is not in the seen-set"; return TLAG_ESTATE; }
+  return TLAG_OK;
+}
+// The CSR keeps the edges it holds, not the bound it was reserved for (kept as it is without memory for the copy)
+static int graph_shrink(tlag_engine* e) {
+  if (e->g_cap <= e->g_edges + e->g_edges / 8 + (1ULL << 20)) return TLAG_OK;
+  const uint64_t cap = e->g_edges ? e->g_edges : 1;
+  uint32_t *nd = nullptr, *na = nullptr;
+  if (dmalloc(e, &nd, cap * 4) != cudaSuccess || dmalloc(e, &na, cap * 4) != cudaSuccess) {
+    cudaGetLastError();
+    dfree(e, nd); dfree(e, na);
+    return TLAG_OK;
+  }
+  CK(cudaMemcpyAsync(nd, e->d_gdst, e->g_edges * 4, cudaMemcpyDeviceToDevice, e->stream));
+  CK(cudaMemcpyAsync(na, e->d_gact, e->g_edges * 4, cudaMemcpyDeviceToDevice, e->stream));
+  dfree(e, e->d_gdst); dfree(e, e->d_gact);
+  e->d_gdst = nd; e->d_gact = na; e->g_cap = cap;
+  return TLAG_OK;
+}
+#endif
+
+extern "C" int tlag_build_graph(tlag_engine* e, tlag_graph_info* out) {
+  if (!e || !out) return TLAG_EINVAL;
+  memset(out, 0, sizeof(*out));
+#if defined(TLAG_SL_SIM)
+  e->err = "this library holds the model's simulation kernels only: the state graph needs its BFS library";
+  return TLAG_EINVAL;
+#else
+  if (e->m.flags & TLAG_F_EXACT) { e->err = "tlag_build_graph: not on a TLAG_F_EXACT (sequential replay) engine"; return TLAG_EINVAL; }
+  if (e->p.n_ranks > 1 || e->q.n_ranks > 1 || e->p2p_slot >= 0) {
+    e->err = "tlag_build_graph: the engine holds one shard of a multi-GPU search";
+    return TLAG_EINVAL;
+  }
+  if (e->h_init.empty()) { e->err = "tlag_build_graph before tlag_seed"; return TLAG_ESTATE; }
+  if (e->verdict == TLAG_V_EVAL_ERROR || e->kg_verdict == TLAG_V_EVAL_ERROR) {
+    e->err = "tlag_build_graph: the search stopped at an evaluation trap, its successor sets are incomplete";
+    return TLAG_ESTATE;
+  }
+  release_graph(e);
+  Counters hc;
+  CK(read_counters(e, &hc));
+  int r = sync_store(e, hc.n_states);
+  if (r) return r;
+  const uint64_t n_states = hc.n_states, n_exp = e->lo;
+  // the graph comes first: the clustering and discovery buffers are allocated again by the next level that needs them,
+  // and the routed-fingerprint cache is only a filter
+  if (!e->disc_open) { dfree(e, e->d_disc); e->d_disc = nullptr; e->disc_bytes = 0; }
+  dfree(e, e->d_sort); e->d_sort = nullptr; e->sort_bytes = 0;
+  dfree(e, e->d_rset); e->d_rset = nullptr; e->rset_bytes = 0;
+  dfree(e, e->d_sent); e->d_sent = nullptr; e->p.sent_cache = nullptr;
+  GraphScratch sc;
+  float ms = 0;
+  r = timed(e, &ms, nullptr, [&] { return graph_passes(e, sc, n_states, n_exp); });
+  dfree(e, sc.row_of_slot); dfree(e, sc.keys); dfree(e, sc.tmp); dfree(e, sc.ctl);
+  if (!r) r = graph_shrink(e);
+  if (r) { cudaStreamSynchronize(e->stream); release_graph(e); return r; }
+  CK(cudaStreamSynchronize(e->stream));
+  e->g_ready = true;
+  out->n_states = n_states; out->n_expanded = n_exp; out->n_edges = e->g_edges; out->device_ms = ms;
+  return TLAG_OK;
+#endif
+}
+
+extern "C" int tlag_read_graph(tlag_engine* e, uint64_t first, uint64_t n, uint64_t* off_out, uint32_t* dst_out,
+                               int32_t* act_out) {
+  if (!e || !off_out) return TLAG_EINVAL;
+  if (!e->g_ready) { e->err = "no state graph: tlag_build_graph first (tlag_seed, tlag_step, tlag_run and tlag_restart release it)"; return TLAG_ESTATE; }
+  if (first > e->g_states || n > e->g_states - first) { e->err = "tlag_read_graph: rows beyond the state graph"; return TLAG_EINVAL; }
+  CK(cudaMemcpyAsync(off_out, e->d_goff + first, (n + 1) * 8, cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaStreamSynchronize(e->stream));
+  const uint64_t o0 = off_out[0], m = off_out[n] - o0;
+  for (uint64_t i = 0; i <= n; ++i) off_out[i] -= o0;
+  if (dst_out && m) CK(cudaMemcpyAsync(dst_out, e->d_gdst + o0, m * 4, cudaMemcpyDeviceToHost, e->stream));
+  if (act_out && m) CK(cudaMemcpyAsync(act_out, e->d_gact + o0, m * 4, cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaStreamSynchronize(e->stream));
+  return TLAG_OK;
+}
+
+extern "C" int tlag_graph_digest(tlag_engine* e, uint64_t* xor_out, uint64_t* sum_out) {
+  if (!e || !xor_out || !sum_out) return TLAG_EINVAL;
+#if defined(TLAG_SL_SIM)
+  e->err = "this library holds the model's simulation kernels only";
+  return TLAG_EINVAL;
+#else
+  if (!e->g_ready) { e->err = "no state graph: tlag_build_graph first"; return TLAG_ESTATE; }
+  if (!e->d_dig) CK(cudaMalloc(&e->d_dig, 16));
+  CK(cudaMemsetAsync(e->d_dig, 0, 16, e->stream));
+  if (e->g_expanded) {
+    k_graph_digest<<<e->sm_count * 8, 256, 0, e->stream>>>(e->p, e->d_goff, e->d_gdst, e->d_gact, e->g_expanded, e->d_dig);
+    e->launches++;
+    CK(cudaGetLastError());
+  }
   unsigned long long h2[2];
   CK(cudaMemcpyAsync(h2, e->d_dig, 16, cudaMemcpyDeviceToHost, e->stream));
   CK(cudaStreamSynchronize(e->stream));

@@ -203,6 +203,13 @@ TLAG_HD uint64_t tlag_sim_term(uint64_t fp, uint64_t w, uint32_t t, int32_t act)
   return tlag_mix64(fp ^ tlag_mix64(w * 0x9E3779B97F4A7C15ULL + ((uint64_t)t << 16) + (uint64_t)(uint16_t)act));
 }
 
+// ---- state graph ---------------------------------------------------------------------
+// One edge s -> t with action id a in the graph digest (tlag_graph_digest), from the fingerprints of its two states: the
+// XOR and the SUM of it over all edges do not depend on the order of the store.
+TLAG_HD uint64_t tlag_edge_term(uint64_t fp_s, uint64_t fp_t, int32_t a) {
+  return tlag_mix64(tlag_mix64(fp_s ^ 0x9E3779B97F4A7C15ULL) ^ tlag_mix64(fp_t + (uint64_t)(uint32_t)a));
+}
+
 // Walks of one batch: min(num, 2^20, what a 4 GiB history holds at depth D), rounded down to a multiple of 32 (at least
 // 32).  It depends on W, D and num only, so a run's batches, and with them its first error, are the same on any GPU.
 #define TLAG_SIM_BUDGET (4ULL << 30)

@@ -61,6 +61,13 @@ class TlagResult(C.Structure):
         return {f: getattr(self, f) for f, _ in self._fields_}
 
 
+class GraphInfo(C.Structure):
+    _fields_ = [("n_states", C.c_uint64), ("n_expanded", C.c_uint64), ("n_edges", C.c_uint64), ("device_ms", C.c_float)]
+
+    def as_dict(self):
+        return {f: getattr(self, f) for f, _ in self._fields_}
+
+
 class SimParams(C.Structure):
     _fields_ = [("seed", C.c_uint64), ("first_walk", C.c_uint64), ("num_walks", C.c_uint64), ("depth", C.c_uint32),
                 ("flags", C.c_uint32)]
@@ -80,7 +87,8 @@ EXPORTS = ["tlag_create", "tlag_seed", "tlag_step", "tlag_run", "tlag_result_now
            "tlag_kernel_launches", "tlag_destroy", "tlag_last_error", "tlag_version",
            "tlag_frontier", "tlag_expand_route", "tlag_insert_records", "tlag_advance_level",
            "tlag_p2p_init", "tlag_p2p_attach", "tlag_p2p_level", "tlag_p2p_rollback", "tlag_read_link", "tlag_set_rank", "tlag_set_owner_words",
-           "tlag_simulate", "tlag_sim_trace", "tlag_sim_read", "tlag_sim_digest"]
+           "tlag_simulate", "tlag_sim_trace", "tlag_sim_read", "tlag_sim_digest",
+           "tlag_build_graph", "tlag_read_graph", "tlag_graph_digest"]
 
 
 def build_library(verbose=False):
@@ -385,6 +393,33 @@ class Engine:
     def sim_digest(self):
         x, s_ = C.c_uint64(), C.c_uint64()
         self._ck(self.L.tlag_sim_digest(self.h, C.byref(x), C.byref(s_)), "tlag_sim_digest")
+        return int(x.value), int(s_.value)
+
+    # state graph (include/tlag.h: tlag_build_graph)
+    def build_graph(self) -> dict:
+        """The state graph of the store, built in device memory.  -> dict(n_states, n_expanded, n_edges, device_ms)"""
+        gi = GraphInfo()
+        self._ck(self.L.tlag_build_graph(self.h, C.byref(gi)), "tlag_build_graph")
+        self._graph_states = gi.n_states
+        return gi.as_dict()
+
+    def state_graph(self, first=0, n=None):
+        """Edges out of rows [first, first + n) (default: to the last row) -> (off [n + 1] uint64 relative to row
+        `first`, dst [off[n]] uint32 rows, act [off[n]] int32 action ids)"""
+        if n is None:
+            n = getattr(self, "_graph_states", 0) - first
+        off = np.zeros(n + 1, dtype=np.uint64)
+        self._ck(self.L.tlag_read_graph(self.h, C.c_uint64(first), C.c_uint64(n), off.ctypes.data_as(C.c_void_p), None, None),
+                 "tlag_read_graph")
+        dst = np.zeros(int(off[-1]), dtype=np.uint32)
+        act = np.zeros(int(off[-1]), dtype=np.int32)
+        self._ck(self.L.tlag_read_graph(self.h, C.c_uint64(first), C.c_uint64(n), off.ctypes.data_as(C.c_void_p),
+                                        dst.ctypes.data_as(C.c_void_p), act.ctypes.data_as(C.c_void_p)), "tlag_read_graph")
+        return off, dst, act
+
+    def graph_digest(self):
+        x, s_ = C.c_uint64(), C.c_uint64()
+        self._ck(self.L.tlag_graph_digest(self.h, C.byref(x), C.byref(s_)), "tlag_graph_digest")
         return int(x.value), int(s_.value)
 
     # multi-GPU building blocks
