@@ -19,6 +19,7 @@
 #include <string.h>
 #include <stdlib.h>
 #include <string>
+#include <type_traits>
 #include <unordered_set>
 #include <vector>
 #include <cub/device/device_radix_sort.cuh>   // CUDA-toolkit header library; used only to reorder a level (not on the hot path)
@@ -39,6 +40,20 @@
 #define TLAG_MAXW 128
 #define TLAG_BLOCK 512
 #define TLAG_MAX_STEPS (1u << 26)
+
+// The policy that picks an interpreter kernel's variant (vm_variant; a sliced library's k_graph at compile time).  The
+// frame is a per-thread array of the frame class: the frame rounded up to a power of two, 64 to 8192 words.
+constexpr int vm_frame_class(uint32_t words) {
+  int c = 64;
+  while (c < 8192 && (uint32_t)c < words) c *= 2;
+  return c;
+}
+// The program runs from shared memory when it fits.  Big frames (container models such as raft) are bound by local-memory
+// latency (ncu: long-scoreboard 37 per issue, 16 warps/SM): they run with the program in global memory (read through L1)
+// so that two CTAs fit per SM.
+constexpr bool vm_code_in_smem(uint32_t words, uint32_t code_len) {
+  return (uint64_t)code_len * 8 <= (words > 512 ? 0 : 200 * 1024);
+}
 
 #define CK(call)                                                                         \
   do {                                                                                   \
@@ -70,7 +85,7 @@ struct tlag_engine {
   cudaStream_t stream = nullptr;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
   int sm_count = 132;
-  int frame_class = 0;
+  int frame_class = 64;              // the interpreter's frame class, in words (vm_frame_class)
   bool uses_ext = false;            // the image contains LEXLT / SFIND / SINS / EMITD (full interpreter needed)
   bool restarting = false;
   bool tight = false;               // TLAG_TIGHT_HEADROOM (test hook): store and table sized for no growth, see read_env_hooks
@@ -119,6 +134,11 @@ struct tlag_engine {
 #ifndef TLAG_SL_BLOCK
 #define TLAG_SL_BLOCK 256
 #endif
+// CTAs of a slice kernel over n rows: one thread per row, at most 64 CTAs per SM
+static unsigned sl_blocks(const tlag_engine* e, uint64_t n) {
+  const uint64_t blocks = (n + TLAG_SL_BLOCK - 1) / TLAG_SL_BLOCK, maxb = (uint64_t)e->sm_count * 64;
+  return (unsigned)(blocks < maxb ? blocks : maxb);
+}
 typedef void (*sl_launch_t)(const DevParams*, unsigned long long, unsigned long long, unsigned, cudaStream_t);
 #ifdef TLAG_SL_SIM
 // a simulation library (build_sliced_library(cm, simulate=True)): its slice kernels are the simulation kernels only
@@ -182,6 +202,50 @@ __device__ __forceinline__ void warp_vm(const uint64_t* __restrict__ gcode, cons
   }
 }
 
+// The program warp_vm fetches from shared memory: with SMEM the CTA copies it there first
+template <bool SMEM>
+__device__ __forceinline__ const uint64_t* vm_stage_code(const DevParams& p) {
+  extern __shared__ uint64_t s_code[];
+  if (SMEM) {
+    for (uint32_t i = threadIdx.x; i < p.code_len; i += blockDim.x) s_code[i] = p.code[i];
+    __syncthreads();
+  }
+  return s_code;
+}
+
+// Row idx of p.states (W = p.W words): its packed words into succ[], unpacked into the frame
+__device__ __forceinline__ void vm_load_row(const DevParams& p, int W, unsigned long long idx, uint32_t* succ,
+                                            int32_t* frame) {
+  const uint32_t* src = p.states + idx * (unsigned long long)W;
+  for (int i = 0; i < W; ++i) succ[i] = src[i];
+  tlag_unpack(p.layout, p.n_slots, succ, frame + p.n_off);
+}
+
+// The successor at the lane's EMIT into succ[]: EMITD (info2 > 0) re-packs its dirty slot ranges into a copy of row idx,
+// EMIT packs the whole frame.  Returns 0, or 1 + the slot whose value does not fit (tlag_pack).
+template <bool LEAN>
+__device__ __forceinline__ int vm_pack_emit(const DevParams& p, int W, unsigned long long idx, int32_t info2,
+                                            const int32_t* frame, uint32_t* succ) {
+  if (!LEAN && info2 > 0) {
+    const uint32_t* src = p.states + idx * (unsigned long long)W;
+    for (int i = 0; i < W; ++i) succ[i] = src[i];
+    return tlag_pack_ranges(p.layout, p.cpool, info2, frame + p.p_off, succ);
+  }
+  return tlag_pack(p.layout, p.n_slots, frame + p.p_off, succ, W);
+}
+
+// v summed over the warp and added to *total, one atomic per warp
+__device__ __forceinline__ void warp_add(unsigned long long* total, unsigned long long v) {
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
+  if ((threadIdx.x & 31) == 0 && v) atomicAdd(total, v);
+}
+
+// A digest kernel's last step: the XOR and the SUM of its terms over the warp, into out2[0] and out2[1]
+__device__ __forceinline__ void warp_digest(unsigned long long* out2, unsigned long long x, unsigned long long sm) {
+  for (int o = 16; o > 0; o >>= 1) { x ^= __shfl_down_sync(0xffffffffu, x, o); sm += __shfl_down_sync(0xffffffffu, sm, o); }
+  if ((threadIdx.x & 31) == 0) { atomicXor(&out2[0], x); atomicAdd(&out2[1], sm); }
+}
+
 #ifndef TLAG_SLICED_INC   // (a sliced library runs the interpreter only in the state graph's edge pass, k_graph)
 
 // MODE 0: fused insert (single GPU).  MODE 1: route successors to per-owner send regions.
@@ -189,11 +253,7 @@ __device__ __forceinline__ void warp_vm(const uint64_t* __restrict__ gcode, cons
 template <int FRAME, int MODE, bool SMEM, bool LEAN = false>
 __global__ void __launch_bounds__(TLAG_BLOCK, TLAG_WAVE_OCC(FRAME, SMEM))
 k_wave(DevParams p, unsigned long long lo, unsigned long long hi) {
-  extern __shared__ uint64_t s_code[];
-  if (SMEM) {
-    for (uint32_t i = threadIdx.x; i < p.code_len; i += blockDim.x) s_code[i] = p.code[i];
-    __syncthreads();
-  }
+  const uint64_t* s_code = vm_stage_code<SMEM>(p);
   const uint64_t* code = p.code;
   int32_t frame[FRAME];
   uint32_t succ[TLAG_MAXW];
@@ -213,11 +273,7 @@ k_wave(DevParams p, unsigned long long lo, unsigned long long hi) {
     if (first >= hi) break;
     const unsigned long long idx = first + lane;
     const bool active = idx < hi && (!exact || lane == 0);
-    if (active) {
-      const uint32_t* src = p.states + idx * (unsigned long long)W;
-      for (int i = 0; i < W; ++i) succ[i] = src[i];
-      tlag_unpack(p.layout, p.n_slots, succ, frame + p.n_off);
-    }
+    if (active) vm_load_row(p, W, idx, succ, frame);
     bool trapped = false;
     int st, ev = 0;
     int32_t info = 0, info2 = 0;
@@ -259,14 +315,7 @@ k_wave(DevParams p, unsigned long long lo, unsigned long long hi) {
       act = info;
       unsigned long long fp = 0;
       if (has) {
-        int ov;
-        if (!LEAN && info2 > 0) {   // EMITD: copy of the parent's packed words, dirty slot ranges re-packed
-          const uint32_t* src = p.states + idx * (unsigned long long)W;
-          for (int i = 0; i < W; ++i) succ[i] = src[i];
-          ov = tlag_pack_ranges(p.layout, p.cpool, info2, frame + p.p_off, succ);
-        } else {
-          ov = tlag_pack(p.layout, p.n_slots, frame + p.p_off, succ, W);
-        }
+        const int ov = vm_pack_emit<LEAN>(p, W, idx, info2, frame, succ);
         if (ov) {
           report_min(&p.ctr->viol_trap, (idx << 20) | (2ULL << 16) | (unsigned)((ov - 1) & 0xFFFF));
           has = false;
@@ -290,9 +339,7 @@ k_wave(DevParams p, unsigned long long lo, unsigned long long hi) {
       if (exact) atomicExch(&p.ctr->stop, 1ULL);
     }
   }
-  // generated counter: warp reduce then one atomic
-  for (int o = 16; o > 0; o >>= 1) gen_local += __shfl_down_sync(0xffffffffu, gen_local, o);
-  if (lane == 0 && gen_local) atomicAdd(&p.ctr->generated, gen_local);
+  warp_add(&p.ctr->generated, gen_local);
 }
 
 // ------------------------------------------------------------------ random simulation, interpreter
@@ -303,11 +350,7 @@ template <int FRAME, bool SMEM, bool LEAN>
 __global__ void __launch_bounds__(TLAG_BLOCK, TLAG_WAVE_OCC(FRAME, SMEM))
 k_sim(DevParams p, SimParams s, unsigned long long hi) {
   if (sim_stopped(s)) return;
-  extern __shared__ uint64_t s_code[];
-  if (SMEM) {
-    for (uint32_t i = threadIdx.x; i < p.code_len; i += blockDim.x) s_code[i] = p.code[i];
-    __syncthreads();
-  }
+  const uint64_t* s_code = vm_stage_code<SMEM>(p);
   const uint64_t* code = p.code;
   int32_t frame[FRAME];
   uint32_t succ[TLAG_MAXW];
@@ -320,11 +363,7 @@ k_sim(DevParams p, SimParams s, unsigned long long hi) {
     const unsigned long long idx = base + lane;
     int stat = idx < hi ? s.status[idx] : SIM_ENDED;
     const bool active = stat != SIM_ENDED;
-    if (active) {
-      const uint32_t* src = p.states + idx * (unsigned long long)W;
-      for (int i = 0; i < W; ++i) succ[i] = src[i];
-      tlag_unpack(p.layout, p.n_slots, succ, frame + p.n_off);
-    }
+    if (active) vm_load_row(p, W, idx, succ, frame);
     int st, ev = 0;
     int32_t info = 0, info2 = 0;
     uint32_t pc, rpc = 0;
@@ -357,14 +396,7 @@ k_sim(DevParams p, SimParams s, unsigned long long hi) {
       if (__any_sync(0xffffffffu, pc != TLAG_PC_PARKED)) continue;
       if (!__any_sync(0xffffffffu, st == L_EMIT)) break;
       if (st == L_EMIT) {
-        int ov;
-        if (!LEAN && info2 > 0) {
-          const uint32_t* src = p.states + idx * (unsigned long long)W;
-          for (int i = 0; i < W; ++i) succ[i] = src[i];
-          ov = tlag_pack_ranges(p.layout, p.cpool, info2, frame + p.p_off, succ);
-        } else {
-          ov = tlag_pack(p.layout, p.n_slots, frame + p.p_off, succ, W);
-        }
+        const int ov = vm_pack_emit<LEAN>(p, W, idx, info2, frame, succ);
         if (ov) {
           report_min(&p.ctr->viol_trap, (idx << 20) | (2ULL << 16) | (unsigned)((ov - 1) & 0xFFFF));
           stat = SIM_FAILED;
@@ -380,8 +412,7 @@ k_sim(DevParams p, SimParams s, unsigned long long hi) {
       if (nsucc) p.succ_flag[idx] = 1;
     }
   }
-  for (int o = 16; o > 0; o >>= 1) gen_local += __shfl_down_sync(0xffffffffu, gen_local, o);
-  if (lane == 0 && gen_local) atomicAdd(&p.ctr->generated, gen_local);
+  warp_add(&p.ctr->generated, gen_local);
 }
 #endif  // !TLAG_SLICED_INC
 
@@ -421,8 +452,7 @@ __global__ void k_sim_end(DevParams p, SimParams s, unsigned long long n) {
     s.status[i] = more ? SIM_RUN : SIM_ENDED;
     s.cnt[i] = 0; p.succ_flag[i] = 0;
   }
-  for (int o = 16; o > 0; o >>= 1) ran += __shfl_down_sync(0xffffffffu, ran, o);
-  if ((threadIdx.x & 31) == 0 && ran) atomicAdd(&s.ctl->checked, ran);
+  warp_add(&s.ctl->checked, ran);
 }
 
 // XOR and SUM over the batch's behaviours: one term per state checked, from its fingerprint, walk, step and action
@@ -437,8 +467,7 @@ __global__ void k_sim_digest(SimParams s, int W, unsigned long long n, unsigned 
                                                s.act[t * s.B + i]);
     x ^= v; sm += v;
   }
-  for (int o = 16; o > 0; o >>= 1) { x ^= __shfl_down_sync(0xffffffffu, x, o); sm += __shfl_down_sync(0xffffffffu, sm, o); }
-  if ((threadIdx.x & 31) == 0) { atomicXor(&out2[0], x); atomicAdd(&out2[1], sm); }
+  warp_digest(out2, x, sm);
 }
 
 #if !defined(TLAG_SL_SIM)
@@ -488,11 +517,7 @@ __global__ void k_graph_index(DevParams p, unsigned long long n, uint32_t* __res
 template <int FRAME, bool SMEM, bool LEAN>
 __global__ void __launch_bounds__(TLAG_BLOCK, TLAG_WAVE_OCC(FRAME, SMEM))
 k_graph(DevParams p, GraphParams g, unsigned long long hi) {
-  extern __shared__ uint64_t s_code[];
-  if (SMEM) {
-    for (uint32_t i = threadIdx.x; i < p.code_len; i += blockDim.x) s_code[i] = p.code[i];
-    __syncthreads();
-  }
+  const uint64_t* s_code = vm_stage_code<SMEM>(p);
   const uint64_t* code = p.code;
   int32_t frame[FRAME];
   uint32_t succ[TLAG_MAXW];
@@ -503,11 +528,7 @@ k_graph(DevParams p, GraphParams g, unsigned long long hi) {
        base += stride) {
     const unsigned long long idx = base + lane;
     const bool active = idx < hi;
-    if (active) {
-      const uint32_t* src = p.states + idx * (unsigned long long)W;
-      for (int i = 0; i < W; ++i) succ[i] = src[i];
-      tlag_unpack(p.layout, p.n_slots, succ, frame + p.n_off);
-    }
+    if (active) vm_load_row(p, W, idx, succ, frame);
     int st = active ? L_RUN : L_DONE, ev = 0;
     int32_t info = 0, info2 = 0;
     uint32_t pc = active ? p.entry_next : TLAG_PC_PARKED, rpc = 0;
@@ -524,14 +545,7 @@ k_graph(DevParams p, GraphParams g, unsigned long long hi) {
       bool keep = false;
       unsigned long long key = 0;
       if (st == L_EMIT) {
-        int ov;
-        if (!LEAN && info2 > 0) {
-          const uint32_t* src = p.states + idx * (unsigned long long)W;
-          for (int i = 0; i < W; ++i) succ[i] = src[i];
-          ov = tlag_pack_ranges(p.layout, p.cpool, info2, frame + p.p_off, succ);
-        } else {
-          ov = tlag_pack(p.layout, p.n_slots, frame + p.p_off, succ, W);
-        }
+        const int ov = vm_pack_emit<LEAN>(p, W, idx, info2, frame, succ);
         if (ov || info < 0 || ((unsigned long long)info >> g.abits) != 0) {
           atomicExch(&g.ctl->bad, 1ULL);
         } else {
@@ -603,8 +617,7 @@ __global__ void k_graph_digest(DevParams p, const unsigned long long* __restrict
       x ^= v; sm += v;
     }
   }
-  for (int o = 16; o > 0; o >>= 1) { x ^= __shfl_down_sync(0xffffffffu, x, o); sm += __shfl_down_sync(0xffffffffu, sm, o); }
-  if ((threadIdx.x & 31) == 0) { atomicXor(&out2[0], x); atomicAdd(&out2[1], sm); }
+  warp_digest(out2, x, sm);
 }
 #endif  // !TLAG_SL_SIM
 
@@ -776,8 +789,7 @@ __global__ void k_digest(DevParams p, unsigned long long n, unsigned long long* 
     const unsigned long long fp = tlag_fingerprint(w, p.W);
     x ^= fp; sm += fp;
   }
-  for (int o = 16; o > 0; o >>= 1) { x ^= __shfl_down_sync(0xffffffffu, x, o); sm += __shfl_down_sync(0xffffffffu, sm, o); }
-  if ((threadIdx.x & 31) == 0) { atomicXor(&out2[0], x); atomicAdd(&out2[1], sm); }
+  warp_digest(out2, x, sm);
 }
 
 // ---- frontier clustering -----------------------------------------------------------------------
@@ -983,7 +995,60 @@ static void point_appends(tlag_engine* e) {
   }
 }
 
-static const int kFrameClasses[] = {64, 128, 256, 512, 1024, 2048, 4096, 8192};
+// Lets kernel fn take `bytes` of dynamic shared memory (past the default 48 KB it has to opt in)
+template <class K>
+static cudaError_t allow_smem(K fn, size_t bytes) {
+  return bytes > 48 * 1024 ? cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes) : cudaSuccess;
+}
+
+// The dynamic shared memory of an interpreter kernel: the program, when the engine's variant runs it from there
+static inline size_t vm_smem(const tlag_engine* e) { return e->p.code_in_smem ? (size_t)e->p.code_len * 8 : 0; }
+
+// Interpreter kernel fn over `rows` rows, one lane per row (k_wave: a warp per 32-row chunk, the same count), on a
+// persistent grid: at most one resident wave of CTAs, at least one CTA
+template <class... P, class... A>
+static cudaError_t launch_vm(tlag_engine* e, void (*fn)(P...), uint64_t rows, const A&... args) {
+  const size_t smem = vm_smem(e);
+  const cudaError_t r = allow_smem(fn, smem);
+  if (r != cudaSuccess) return r;
+  int occ = 1;
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, fn, TLAG_BLOCK, smem) != cudaSuccess || occ < 1) occ = 1;
+  uint64_t blocks = (rows + TLAG_BLOCK - 1) / TLAG_BLOCK;
+  if (blocks > (uint64_t)e->sm_count * (uint64_t)occ) blocks = (uint64_t)e->sm_count * (uint64_t)occ;
+  if (blocks == 0) blocks = 1;
+  fn<<<(unsigned)blocks, TLAG_BLOCK, smem, e->stream>>>(args...);
+  e->launches++;
+  return cudaGetLastError();
+}
+
+// The engine's variant of an interpreter kernel template: its frame class, the program in shared memory or not, and up to
+// 512 words the lean interpreter for a program without the extension ops.  kernel(frame, smem, lean) names the template's
+// instantiation for one variant (each argument a std::integral_constant), so each template gets the 24 variants.
+template <int FRAME, class K>
+static auto vm_variant_of(const tlag_engine* e, K kernel) {
+  using F = std::integral_constant<int, FRAME>;
+  using Y = std::true_type;
+  using N = std::false_type;
+  const bool sm = e->p.code_in_smem != 0;
+  if constexpr (FRAME <= 512)
+    if (!e->uses_ext) return sm ? kernel(F{}, Y{}, Y{}) : kernel(F{}, N{}, Y{});
+  return sm ? kernel(F{}, Y{}, N{}) : kernel(F{}, N{}, N{});
+}
+
+template <class K>
+static auto vm_variant(const tlag_engine* e, K kernel) {
+  switch (e->frame_class) {
+    case 64: return vm_variant_of<64>(e, kernel);
+    case 128: return vm_variant_of<128>(e, kernel);
+    case 256: return vm_variant_of<256>(e, kernel);
+    case 512: return vm_variant_of<512>(e, kernel);
+    case 1024: return vm_variant_of<1024>(e, kernel);
+    case 2048: return vm_variant_of<2048>(e, kernel);
+    case 4096: return vm_variant_of<4096>(e, kernel);
+    // 8192 words = 32 KB of local memory per thread (SSI at 4 transactions x 3 keys needs 6.9 K words)
+    default: return vm_variant_of<8192>(e, kernel);
+  }
+}
 
 #ifdef TLAG_SLICED_INC
 // One BFS level (or one chunk of it, route mode) = the invariant kernels, the kernels of the slices of Next, and the
@@ -1006,59 +1071,27 @@ static cudaError_t launch_wave(tlag_engine* e, uint64_t lo, uint64_t hi) {
   }
   e->p.succ_flag = dl ? e->d_succ : nullptr;
   e->p.route = MODE;
-  uint64_t blocks = (n + TLAG_SL_BLOCK - 1) / TLAG_SL_BLOCK;
-  const uint64_t maxb = (uint64_t)e->sm_count * 64;
-  if (blocks > maxb) blocks = maxb;
+  const unsigned blocks = sl_blocks(e, n);
   if (e->p.n_inv > 0)
-    for (int j = 0; kSlInv[j]; ++j) { kSlInv[j](&e->p, lo, hi, (unsigned)blocks, e->stream); e->launches++; }
-  for (int j = 0; kSlNext[j]; ++j) { kSlNext[j](&e->p, lo, hi, (unsigned)blocks, e->stream); e->launches++; }
+    for (int j = 0; kSlInv[j]; ++j) { kSlInv[j](&e->p, lo, hi, blocks, e->stream); e->launches++; }
+  for (int j = 0; kSlNext[j]; ++j) { kSlNext[j](&e->p, lo, hi, blocks, e->stream); e->launches++; }
   if (dl) { k_sl_deadlock<<<(unsigned)((n + 255) / 256), 256, 0, e->stream>>>(e->p, lo, hi); e->launches++; }
   return cudaGetLastError();
 }
 #else
 template <int MODE>
 static cudaError_t launch_wave(tlag_engine* e, uint64_t lo, uint64_t hi) {
-  const uint64_t n = hi - lo;
-  uint64_t chunks = (n + 31) / 32;
-  uint64_t blocks = (chunks + (TLAG_BLOCK / 32) - 1) / (TLAG_BLOCK / 32);
-  if (blocks == 0) blocks = 1;
-  size_t smem = e->p.code_in_smem ? (size_t)e->p.code_len * 8 : 0;
-  void (*fn)(DevParams, unsigned long long, unsigned long long) = nullptr;
-  const bool sm = e->p.code_in_smem != 0;
-  const bool lean = !e->uses_ext;
-  switch (e->frame_class) {
-    case 0: fn = lean ? (sm ? k_wave<64, MODE, true, true> : k_wave<64, MODE, false, true>)
-                      : (sm ? k_wave<64, MODE, true> : k_wave<64, MODE, false>); break;
-    case 1: fn = lean ? (sm ? k_wave<128, MODE, true, true> : k_wave<128, MODE, false, true>)
-                      : (sm ? k_wave<128, MODE, true> : k_wave<128, MODE, false>); break;
-    case 2: fn = lean ? (sm ? k_wave<256, MODE, true, true> : k_wave<256, MODE, false, true>)
-                      : (sm ? k_wave<256, MODE, true> : k_wave<256, MODE, false>); break;
-    case 3: fn = lean ? (sm ? k_wave<512, MODE, true, true> : k_wave<512, MODE, false, true>)
-                      : (sm ? k_wave<512, MODE, true> : k_wave<512, MODE, false>); break;
-    case 4: fn = sm ? k_wave<1024, MODE, true> : k_wave<1024, MODE, false>; break;
-    case 5: fn = sm ? k_wave<2048, MODE, true> : k_wave<2048, MODE, false>; break;
-    case 6: fn = sm ? k_wave<4096, MODE, true> : k_wave<4096, MODE, false>; break;
-    // 8192 words = 32 KB of local memory per thread (SSI at 4 transactions x 3 keys needs 6.9 K words)
-    default: fn = sm ? k_wave<8192, MODE, true> : k_wave<8192, MODE, false>; break;
-  }
-  if (smem > 48 * 1024) {
-    cudaError_t r = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (r != cudaSuccess) return r;
-  }
-  int occ = 1;
-  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, fn, TLAG_BLOCK, smem) != cudaSuccess || occ < 1) occ = 1;
-  const uint64_t maxb = (uint64_t)e->sm_count * (uint64_t)occ;   // persistent grid: one resident wave of CTAs
-  if (blocks > maxb) blocks = maxb;
+  const auto fn = vm_variant(e, [](auto f, auto s, auto l) { return k_wave<f, MODE, s, l>; });
   if (MODE == 0 && (e->p.flags & TLAG_F_EXACT)) {                 // sequential replay: one warp, one state at a time
+    const size_t smem = vm_smem(e);
+    const cudaError_t r = allow_smem(fn, smem);
+    if (r != cudaSuccess) return r;
     fn<<<1, 32, smem, e->stream>>>(e->p, lo, hi);
     e->launches++;
     return cudaGetLastError();
   }
-  fn<<<(unsigned)blocks, TLAG_BLOCK, smem, e->stream>>>(e->p, lo, hi);
-  e->launches++;
-  return cudaGetLastError();
+  return launch_vm(e, fn, hi - lo, e->p, lo, hi);
 }
-
 #endif
 
 // The counter block after everything queued on the engine's stream so far.  The stream is non-blocking, so a copy on
@@ -1089,6 +1122,20 @@ static int timed(tlag_engine* e, float* ms, Counters* hc, F&& enqueue) {
   if (hc) CK(read_counters(e, hc));
   else CK(cudaEventSynchronize(e->ev1));
   CK(cudaEventElapsedTime(ms, e->ev0, e->ev1));
+  return TLAG_OK;
+}
+
+// The XOR and the SUM a digest kernel accumulates: launch() enqueues it on the engine's stream, into e->d_dig zeroed first
+template <class F>
+static int read_digest(tlag_engine* e, uint64_t* xor_out, uint64_t* sum_out, F&& launch) {
+  if (!e->d_dig) CK(cudaMalloc(&e->d_dig, 16));
+  CK(cudaMemsetAsync(e->d_dig, 0, 16, e->stream));
+  const int r = launch();
+  if (r) return r;
+  unsigned long long h2[2];
+  CK(cudaMemcpyAsync(h2, e->d_dig, 16, cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaStreamSynchronize(e->stream));
+  *xor_out = h2[0]; *sum_out = h2[1];
   return TLAG_OK;
 }
 
@@ -1455,8 +1502,12 @@ extern "C" int tlag_create(const tlag_model* m, tlag_engine** out) {
   }
   CK(cudaEventCreate(&e->ev0));
   CK(cudaEventCreate(&e->ev1));
-  e->frame_class = 7;
-  for (int i = 0; i < 8; ++i) if ((int)m->frame_words <= kFrameClasses[i]) { e->frame_class = i; break; }
+#if defined(TLAG_SLICED_INC)
+  const uint32_t vm_frame = TLAG_SL_FRAME;   // the frame the library's one interpreter kernel is compiled for (launch_graph)
+#else
+  const uint32_t vm_frame = m->frame_words;
+#endif
+  e->frame_class = vm_frame_class(vm_frame);
   for (uint32_t i = 0; i < m->code_len && !e->uses_ext; ++i) {
     const uint32_t op = (uint32_t)(m->code[i] & 0xFF);
     if (op == OP_LEXLT || op == OP_SFIND || op == OP_SINS || op == OP_EMITD || op == OP_CALL || op == OP_RET) e->uses_ext = true;
@@ -1483,11 +1534,7 @@ extern "C" int tlag_create(const tlag_model* m, tlag_engine** out) {
   CK(dmalloc(e, &e->d_parent, cap * 4));
   CK(dmalloc(e, &e->d_meta, cap * 4));
   e->p.code = e->d_code; e->p.code_len = m->code_len;
-  // bytecode image in shared memory when it fits.  Big frames (container models such as raft) are bound by local-memory
-  // latency (ncu: long-scoreboard 37 per issue, 16 warps/SM): they run with the image in global memory (read through L1)
-  // so that two CTAs fit per SM.
-  const size_t smem_lim = m->frame_words > 512 ? 0 : 200 * 1024;
-  e->p.code_in_smem = ((size_t)m->code_len * 8 <= smem_lim) ? 1 : 0;
+  e->p.code_in_smem = vm_code_in_smem(vm_frame, m->code_len) ? 1 : 0;
   e->p.cpool = e->d_cpool; e->p.layout = e->d_layout; e->p.n_slots = (int)m->n_slots;
   e->p.entry_inv = m->entry_inv; e->p.entry_next = m->entry_next;
   e->p.n_off = 0; e->p.p_off = m->unpacked_words; e->p.W = (int)m->words_per_state;
@@ -1544,7 +1591,7 @@ static int launch_probe(tlag_engine* e, const uint32_t* d_states, uint64_t n, ui
   if (n == 0) return TLAG_OK;
   if (((uintptr_t)d_states % 16) == 0 && W >= 2) {
     const size_t smem = (size_t)256 * (size_t)(W | 1) * 4;
-    if (smem > 48 * 1024) CK(cudaFuncSetAttribute(k_probe_staged, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    CK(allow_smem(k_probe_staged, smem));
     k_probe_staged<<<blocks, 256, smem, e->stream>>>(d_states, n, W, e->d_table, e->p.mask, d_is_new, e->d_ctr);
   } else {
     k_probe<<<blocks, 256, 0, e->stream>>>(d_states, n, W, e->d_table, e->p.mask, d_is_new, e->d_ctr);
@@ -1860,19 +1907,14 @@ extern "C" int tlag_digest(tlag_engine* e, uint64_t* xor_out, uint64_t* sum_out)
   CK(read_counters(e, &hc));
   int r = sync_store(e, hc.n_states);
   if (r) return r;
-  if (!e->d_dig) CK(cudaMalloc(&e->d_dig, 16));
-  unsigned long long* d2 = e->d_dig;
-  CK(cudaMemsetAsync(d2, 0, 16, e->stream));
-  if (hc.n_states) {
-    k_digest<<<e->sm_count * 8, 256, 0, e->stream>>>(e->p, hc.n_states, d2);
-    e->launches++;
-    CK(cudaGetLastError());
-  }
-  unsigned long long h2[2];
-  CK(cudaMemcpyAsync(h2, d2, 16, cudaMemcpyDeviceToHost, e->stream));
-  CK(cudaStreamSynchronize(e->stream));
-  *xor_out = h2[0]; *sum_out = h2[1];
-  return TLAG_OK;
+  return read_digest(e, xor_out, sum_out, [&] {
+    if (hc.n_states) {
+      k_digest<<<e->sm_count * 8, 256, 0, e->stream>>>(e->p, hc.n_states, e->d_dig);
+      e->launches++;
+      CK(cudaGetLastError());
+    }
+    return TLAG_OK;
+  });
 }
 
 // One hop of a counterexample chain: the state at idx (when state_out) with its parent index and meta word (action id
@@ -2187,41 +2229,16 @@ extern "C" int tlag_advance_level(tlag_engine* e, tlag_wave_stats* out) {
 #if defined(TLAG_SLICED_INC)
 #if defined(TLAG_SL_SIM)
 static cudaError_t launch_sim_step(tlag_engine* e, const DevParams& p, const SimParams& s, uint64_t n) {
-  uint64_t blocks = (n + TLAG_SL_BLOCK - 1) / TLAG_SL_BLOCK;
-  if (blocks > (uint64_t)e->sm_count * 64) blocks = (uint64_t)e->sm_count * 64;
+  const unsigned blocks = sl_blocks(e, n);
   if (p.n_inv > 0)
-    for (int j = 0; kSlSimInv[j]; ++j) { kSlSimInv[j](&p, &s, n, (unsigned)blocks, e->stream); e->launches++; }
-  for (int j = 0; kSlSimNext[j]; ++j) { kSlSimNext[j](&p, &s, n, (unsigned)blocks, e->stream); e->launches++; }
+    for (int j = 0; kSlSimInv[j]; ++j) { kSlSimInv[j](&p, &s, n, blocks, e->stream); e->launches++; }
+  for (int j = 0; kSlSimNext[j]; ++j) { kSlSimNext[j](&p, &s, n, blocks, e->stream); e->launches++; }
   return cudaGetLastError();
 }
 #endif
 #else
 static cudaError_t launch_sim_step(tlag_engine* e, const DevParams& p, const SimParams& s, uint64_t n) {
-  const size_t smem = p.code_in_smem ? (size_t)p.code_len * 8 : 0;
-  void (*fn)(DevParams, SimParams, unsigned long long) = nullptr;
-  const bool sm = p.code_in_smem != 0;
-  const bool lean = !e->uses_ext;
-  switch (e->frame_class) {
-    case 0: fn = lean ? (sm ? k_sim<64, true, true> : k_sim<64, false, true>) : (sm ? k_sim<64, true, false> : k_sim<64, false, false>); break;
-    case 1: fn = lean ? (sm ? k_sim<128, true, true> : k_sim<128, false, true>) : (sm ? k_sim<128, true, false> : k_sim<128, false, false>); break;
-    case 2: fn = lean ? (sm ? k_sim<256, true, true> : k_sim<256, false, true>) : (sm ? k_sim<256, true, false> : k_sim<256, false, false>); break;
-    case 3: fn = lean ? (sm ? k_sim<512, true, true> : k_sim<512, false, true>) : (sm ? k_sim<512, true, false> : k_sim<512, false, false>); break;
-    case 4: fn = sm ? k_sim<1024, true, false> : k_sim<1024, false, false>; break;
-    case 5: fn = sm ? k_sim<2048, true, false> : k_sim<2048, false, false>; break;
-    case 6: fn = sm ? k_sim<4096, true, false> : k_sim<4096, false, false>; break;
-    default: fn = sm ? k_sim<8192, true, false> : k_sim<8192, false, false>; break;
-  }
-  if (smem > 48 * 1024) {
-    cudaError_t r = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (r != cudaSuccess) return r;
-  }
-  int occ = 1;
-  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, fn, TLAG_BLOCK, smem) != cudaSuccess || occ < 1) occ = 1;
-  uint64_t blocks = (n + TLAG_BLOCK - 1) / TLAG_BLOCK;
-  if (blocks > (uint64_t)e->sm_count * (uint64_t)occ) blocks = (uint64_t)e->sm_count * (uint64_t)occ;
-  fn<<<(unsigned)blocks, TLAG_BLOCK, smem, e->stream>>>(p, s, n);
-  e->launches++;
-  return cudaGetLastError();
+  return launch_vm(e, vm_variant(e, [](auto f, auto sm, auto l) { return k_sim<f, sm, l>; }), n, p, s, n);
 }
 #endif
 
@@ -2396,80 +2413,28 @@ extern "C" int tlag_sim_digest(tlag_engine* e, uint64_t* xor_out, uint64_t* sum_
   return TLAG_EINVAL;
 #else
   if (!e->sim_n) { e->err = "tlag_sim_digest before tlag_simulate"; return TLAG_ESTATE; }
-  if (!e->d_dig) CK(cudaMalloc(&e->d_dig, 16));
-  CK(cudaMemsetAsync(e->d_dig, 0, 16, e->stream));
   tlag_sim_params sp;
   memset(&sp, 0, sizeof(sp));
   sp.depth = (uint32_t)e->sim_D;
   const SimParams s = sim_params(e, &sp, e->sim_first);
-  k_sim_digest<<<e->sm_count * 8, 256, 0, e->stream>>>(s, (int)e->m.words_per_state, e->sim_n, e->d_dig);
-  e->launches++;
-  CK(cudaGetLastError());
-  unsigned long long h2[2];
-  CK(cudaMemcpyAsync(h2, e->d_dig, 16, cudaMemcpyDeviceToHost, e->stream));
-  CK(cudaStreamSynchronize(e->stream));
-  *xor_out = h2[0]; *sum_out = h2[1];
-  return TLAG_OK;
+  return read_digest(e, xor_out, sum_out, [&] {
+    k_sim_digest<<<e->sm_count * 8, 256, 0, e->stream>>>(s, (int)e->m.words_per_state, e->sim_n, e->d_dig);
+    e->launches++;
+    CK(cudaGetLastError());
+    return TLAG_OK;
+  });
 #endif
 }
 
 // ---- state graph (include/tlag.h: tlag_build_graph) -------------------------------------------------------------------
 #if !defined(TLAG_SL_SIM)
-#if defined(TLAG_SLICED_INC)
-// a sliced library holds one variant of the edge pass: the frame class of its model and, as tlag_create decides for the
-// interpreter, the program in shared memory when it fits
-#if TLAG_SL_FRAME <= 64
-#define TLAG_GRAPH_FRAME 64
-#elif TLAG_SL_FRAME <= 128
-#define TLAG_GRAPH_FRAME 128
-#elif TLAG_SL_FRAME <= 256
-#define TLAG_GRAPH_FRAME 256
-#elif TLAG_SL_FRAME <= 512
-#define TLAG_GRAPH_FRAME 512
-#elif TLAG_SL_FRAME <= 1024
-#define TLAG_GRAPH_FRAME 1024
-#elif TLAG_SL_FRAME <= 2048
-#define TLAG_GRAPH_FRAME 2048
-#elif TLAG_SL_FRAME <= 4096
-#define TLAG_GRAPH_FRAME 4096
-#else
-#define TLAG_GRAPH_FRAME 8192
-#endif
-#define TLAG_GRAPH_SMEM (TLAG_SL_FRAME <= 512 && TLAG_NATIVE_CODE_LEN * 8ull <= 200ull * 1024)
-#endif
-
 static cudaError_t launch_graph(tlag_engine* e, const GraphParams& g, uint64_t hi) {
-  void (*fn)(DevParams, GraphParams, unsigned long long) = nullptr;
-#if defined(TLAG_SLICED_INC)
-  const bool sm = TLAG_GRAPH_SMEM;
-  fn = k_graph<TLAG_GRAPH_FRAME, TLAG_GRAPH_SMEM, false>;
+#if defined(TLAG_SLICED_INC)   // the one variant of the edge pass the policy picks for the library's model
+  const auto fn = k_graph<vm_frame_class(TLAG_SL_FRAME), vm_code_in_smem(TLAG_SL_FRAME, TLAG_NATIVE_CODE_LEN), false>;
 #else
-  const bool sm = e->p.code_in_smem != 0;
-  const bool lean = !e->uses_ext;
-  switch (e->frame_class) {
-    case 0: fn = lean ? (sm ? k_graph<64, true, true> : k_graph<64, false, true>) : (sm ? k_graph<64, true, false> : k_graph<64, false, false>); break;
-    case 1: fn = lean ? (sm ? k_graph<128, true, true> : k_graph<128, false, true>) : (sm ? k_graph<128, true, false> : k_graph<128, false, false>); break;
-    case 2: fn = lean ? (sm ? k_graph<256, true, true> : k_graph<256, false, true>) : (sm ? k_graph<256, true, false> : k_graph<256, false, false>); break;
-    case 3: fn = lean ? (sm ? k_graph<512, true, true> : k_graph<512, false, true>) : (sm ? k_graph<512, true, false> : k_graph<512, false, false>); break;
-    case 4: fn = sm ? k_graph<1024, true, false> : k_graph<1024, false, false>; break;
-    case 5: fn = sm ? k_graph<2048, true, false> : k_graph<2048, false, false>; break;
-    case 6: fn = sm ? k_graph<4096, true, false> : k_graph<4096, false, false>; break;
-    default: fn = sm ? k_graph<8192, true, false> : k_graph<8192, false, false>; break;
-  }
+  const auto fn = vm_variant(e, [](auto f, auto s, auto l) { return k_graph<f, s, l>; });
 #endif
-  const size_t smem = sm ? (size_t)e->p.code_len * 8 : 0;
-  if (smem > 48 * 1024) {
-    cudaError_t r = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (r != cudaSuccess) return r;
-  }
-  int occ = 1;
-  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, fn, TLAG_BLOCK, smem) != cudaSuccess || occ < 1) occ = 1;
-  uint64_t blocks = (hi - g.first + TLAG_BLOCK - 1) / TLAG_BLOCK;
-  if (blocks > (uint64_t)e->sm_count * (uint64_t)occ) blocks = (uint64_t)e->sm_count * (uint64_t)occ;
-  if (blocks == 0) blocks = 1;
-  fn<<<(unsigned)blocks, TLAG_BLOCK, smem, e->stream>>>(e->p, g, hi);
-  e->launches++;
-  return cudaGetLastError();
+  return launch_vm(e, fn, hi - g.first, e->p, g, hi);
 }
 
 static unsigned bits_for(uint64_t n) {   // bits of n - 1, at least 1
@@ -2706,17 +2671,13 @@ extern "C" int tlag_graph_digest(tlag_engine* e, uint64_t* xor_out, uint64_t* su
   return TLAG_EINVAL;
 #else
   if (!e->g_ready) { e->err = "no state graph: tlag_build_graph first"; return TLAG_ESTATE; }
-  if (!e->d_dig) CK(cudaMalloc(&e->d_dig, 16));
-  CK(cudaMemsetAsync(e->d_dig, 0, 16, e->stream));
-  if (e->g_expanded) {
-    k_graph_digest<<<e->sm_count * 8, 256, 0, e->stream>>>(e->p, e->d_goff, e->d_gdst, e->d_gact, e->g_expanded, e->d_dig);
-    e->launches++;
-    CK(cudaGetLastError());
-  }
-  unsigned long long h2[2];
-  CK(cudaMemcpyAsync(h2, e->d_dig, 16, cudaMemcpyDeviceToHost, e->stream));
-  CK(cudaStreamSynchronize(e->stream));
-  *xor_out = h2[0]; *sum_out = h2[1];
-  return TLAG_OK;
+  return read_digest(e, xor_out, sum_out, [&] {
+    if (e->g_expanded) {
+      k_graph_digest<<<e->sm_count * 8, 256, 0, e->stream>>>(e->p, e->d_goff, e->d_gdst, e->d_gact, e->g_expanded, e->d_dig);
+      e->launches++;
+      CK(cudaGetLastError());
+    }
+    return TLAG_OK;
+  });
 #endif
 }
