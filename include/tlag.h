@@ -195,6 +195,41 @@ int  tlag_read_graph(tlag_engine *e, uint64_t first, uint64_t n, uint64_t *off_o
  * fingerprints of s and t and on a: does not depend on the store's order. */
 int  tlag_graph_digest(tlag_engine *e, uint64_t *xor_out, uint64_t *sum_out);
 
+/* ---- liveness labels of the state graph (DESIGN.md §7h) ---------------------------------------------------------------
+ * tlag_label_graph runs a label image (compile/lower.py compile_labels: its own bytecode and constant pool over the model's
+ * layout and frame) on the graph tlag_build_graph left: the state program on every stored row (state word bit j = state
+ * predicate j holds), the edge program on every edge (s, t) with s in the current frame and t in the primed one (edge word
+ * bit j = <<A_j>>_v holds), each predicate that is false raising INVF j.  Then, for every edge bit b, en_bit[b] (< 32) is
+ * set in the state word of each row with an out-edge that has bit b (ENABLED <<A_b>>_v over the stored successors: see
+ * DESIGN.md §7h), nen_bit[b] (< 32) in the state word of each row without one; 0xFF = not derived.  A program that traps
+ * on a row or an edge is TLAG_EEVAL.  The labels belong to the graph and are released with it; labelling again replaces
+ * them.  device_ms: the two label passes and the ENABLED pass (CUDA events). */
+typedef struct {
+  const uint64_t *code;          /* the label image, copied                                     */
+  uint32_t code_len;
+  uint32_t entry_states;         /* pc of the state program                                     */
+  uint32_t entry_edges;          /* pc of the edge program                                      */
+  uint32_t n_state_preds;        /* state bits [0, n) the state program writes (<= 32)           */
+  uint32_t n_edge_preds;         /* edge bits [0, n) the edge program writes (<= 32)             */
+  const int32_t *cpool;          /* the image's constant pool, copied                           */
+  uint32_t cpool_len;
+  uint8_t  en_bit[32], nen_bit[32];
+} tlag_label_program;
+
+int  tlag_label_graph(tlag_engine *e, const tlag_label_program *prog, float *device_ms);
+
+/* The engine's graph as device pointers (as tlag_expand_route takes them), valid until the graph is released: the CSR
+ * (off: n_states + 1 uint64, dst: n_edges uint32), the labels (state_label: n_states uint32, edge_label: n_edges uint32,
+ * 0 when not labelled), the device, and n_init: rows [0, n_init) are the initial states. */
+typedef struct {
+  uint64_t n_states, n_edges;
+  uint64_t off, dst, state_label, edge_label;
+  uint64_t n_init;
+  int32_t  device;
+} tlag_graph_dev;
+
+int  tlag_graph_view(tlag_engine *e, tlag_graph_dev *out);
+
 /* ---- multi-GPU building blocks (one engine per rank; the host exchanges the buffers,
  *      e.g. torch.distributed all_to_all_single over NCCL/NVLink; SURVEY.md §8e) ---------- */
 /* Expand the current frontier WITHOUT inserting: successor records (W state words + parent
@@ -287,9 +322,44 @@ typedef struct {
  * and C holds a state with each need_clear bit clear.  C failing a WF or need_clear test is dropped; C failing only
  * SF tests loses its EN states and the rest is decomposed again, to a fixpoint.  scc_out[v] = accepted SCC id of v,
  * else 0xFFFFFFFF (NULL: not returned).  The cycle through every state and edge of an accepted SCC is fair and
- * violates the obligation the masks and need_clear encode.  Provisional: it uploads the graph and builds both CSRs on
- * every call; the obligation check on a graph the engine builds in device memory will replace it. */
+ * violates the obligation the masks and need_clear encode.  It uploads the graph and builds both CSRs on every call;
+ * tlag_live_check runs the same search on a graph the engine built in device memory. */
 int  tlag_fair_cycles(const tlag_graph *g, const tlag_fair_query *q, uint32_t *scc_out, tlag_fair_result *out);
+
+/* Obligation check on an engine's labelled graph (DESIGN.md §7h), with the decomposition and the Emerson-Lei loop of
+ * tlag_fair_cycles.  The restricted graph keeps the rows whose state word has every keep_set bit and no keep_clear bit,
+ * and the edges between them whose edge word has no edge_drop bit.  Seeds are the rows below seed_rows (0: all rows)
+ * whose state word has every seed_set bit and no seed_clear bit.  With TLAG_LIVE_SEEDS only accepted SCCs reachable from a
+ * seed in the restricted graph count; with TLAG_LIVE_ANY_SEED no SCC is searched and the obligation fails iff a seed
+ * exists ([]P: the rows with ~P), the witness being the smallest.  fair: enabled_bit / action_bit are state / edge bits.
+ * A graph of 2^32 edges or more is TLAG_EINVAL.
+ * For a violation lasso_out receives prefix_len + cycle_len rows: the prefix, a path of the restricted graph from a seed
+ * (without seeds: the witness alone) to the witness, then the cycle, from the witness through an edge with each
+ * condition's action bit (or a ~EN state of a WF condition) and a state with each need_clear bit clear, inside the
+ * accepted SCC, back to (not including) the witness.  cycle_len 1: the SCC is the witness alone, the behaviour stutters
+ * there.  With TLAG_LIVE_ANY_SEED the cycle is empty.  lasso_cap too small: TLAG_EOVERFLOW, lengths set. */
+enum { TLAG_LIVE_SEEDS = 1u, TLAG_LIVE_ANY_SEED = 2u };
+typedef struct {
+  const tlag_fairness *fair;
+  uint32_t n_fair;
+  uint32_t flags;                /* TLAG_LIVE_*                                                 */
+  uint32_t keep_set, keep_clear, edge_drop, need_clear;
+  uint32_t seed_set, seed_clear;
+  uint64_t seed_rows;
+} tlag_live_query;
+
+typedef struct {
+  int32_t  violated;
+  uint32_t witness;              /* smallest row of a (reachable) accepted SCC, or the smallest seed (0xFFFFFFFF: none) */
+  uint64_t fair_sccs;            /* accepted SCCs, reachable or not                             */
+  uint32_t rounds;
+  uint32_t prefix_len, cycle_len;
+  uint32_t reserved;
+  float    check_ms, lasso_ms;   /* device time of the check (from the restriction on) and of the lasso (CUDA events) */
+} tlag_live_result;
+
+int  tlag_live_check(const tlag_graph_dev *g, const tlag_live_query *q, uint32_t *lasso_out, uint32_t lasso_cap,
+                     tlag_live_result *out);
 const char *tlag_graph_last_error(void);
 
 #ifdef __cplusplus

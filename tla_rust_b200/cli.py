@@ -152,7 +152,12 @@ def check_file(path, deadlock=True, cfg_path=None, out=None, device=0, seq_cap=N
     finally:
         _types.SPARSE_CAP = base_sparse
     if simulate is not None:
+        if m.obligations:
+            print("Warning: the temporal properties are not checked in simulation mode.", file=out)
         return _report_simulation(path, m, cm, r, e, simulate[1], t0, out)
+    live = None
+    if m.obligations and r["verdict"] == 0:
+        live = _check_liveness(e, m, cm, r, max_depth, out)
     dumped = _dump(e, cm, m, levels, *dump) if dump is not None else None
     if int(os.environ.get("WORLD_SIZE", "1")) == 1:
         # The parallel search reports an error with the counts of the whole level it was found in, and with whichever of
@@ -170,6 +175,8 @@ def check_file(path, deadlock=True, cfg_path=None, out=None, device=0, seq_cap=N
     if n_out:
         r = dict(r, generated=r["generated"] + n_out, distinct=r["distinct"] + n_out, init_states=r.get("init_states", 0) + n_out)
     res = result_from_engine(cm, r, trace)
+    if live is not None:
+        res = live(res)
     text = format_result(res, m.vars, m.module_name)
     print(text, file=out)
     _write_reports(path, m, res, text)
@@ -179,6 +186,50 @@ def check_file(path, deadlock=True, cfg_path=None, out=None, device=0, seq_cap=N
           f"{e.launches()} kernel launches).", file=out)
     e.close()
     return 0 if res.verdict == OK else 12
+
+
+def _check_liveness(e, m, cm, r, max_depth, out):
+    """The temporal obligations of the model on the search's state graph (DESIGN.md §7h), after a search that reached
+    its fixpoint without an error.  -> None when they hold or were not checked, else the function that turns the
+    search's result into the violation's report"""
+    from . import liveness
+    from .checker import decode_state
+    from .front.report import INVARIANT, LIVENESS
+    why = None
+    if m.fairness_unknown:
+        why = "(the fairness of the SPECIFICATION is not fully understood, see the warning above)"
+    elif m.symmetry:
+        why = "under SYMMETRY (unsound there, as in TLC)"
+    elif int(os.environ.get("WORLD_SIZE", "1")) > 1:
+        why = "on a search spread over several GPUs"
+    elif max_depth and r["queue_left"]:
+        why = "after a depth-bounded search"
+    if why is not None:
+        print(f"Warning: the temporal properties are not checked {why}.", file=out)
+        return None
+    print(f"Checking temporal properties for the complete state space with {r['distinct']} total distinct states.",
+          file=out)
+    found = liveness.check(e, m, cm, lambda w: print(f"Warning: {w}", file=out))
+    if found is None:
+        return None
+    ob, lr = found
+    trace, back, back_act = liveness.lasso(e, lr)
+
+    def label(a):
+        if a is None or a < 0:
+            return None
+        nm, loc, mod = cm.actions[a]
+        return ("fixed", nm, loc, mod)
+
+    def report(res):
+        res.trace = [(decode_state(cm, w), label(a)) for w, a in trace]
+        if ob.kind == "always":
+            res.verdict, res.invariant = INVARIANT, ob.name
+        else:
+            res.verdict = LIVENESS
+            res.back_to = None if back is None else (back + 1, label(back_act))
+        return res
+    return report
 
 
 def _dump(e, cm, m, levels, path, dot):

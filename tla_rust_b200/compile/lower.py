@@ -4445,6 +4445,51 @@ class Lowering:
         cm.state_bits = bits
         return cm
 
+    def _compile_labels(self, cm, state_preds, edge_preds) -> "LabelImage":
+        """compile_labels: the two label programs over cm's frame layout (the offsets of _compile_pass)"""
+        m = self.m
+        self.n_off, self.p_off = dict(cm.var_off), {v: cm.state_words_unpacked + cm.var_off[v] for v in m.vars}
+        self.usz = usz = cm.state_words_unpacked
+        self.blocks = set()
+        for v in m.vars:
+            self.blocks.add((self.n_off[v], self.var_types[v].size))
+            self.blocks.add((self.p_off[v], self.var_types[v].size))
+        self.top = self.high = 2 * usz
+        self._canon = None
+        allv = frozenset(m.vars)
+        entries = {}
+        for prog, preds, bound in (("states", state_preds, frozenset()), ("edges", edge_preds, allv)):
+            lab = Label(prog)
+            self.asm.label(lab)
+            entries[prog] = lab
+            self.program = prog
+            for j, p in enumerate(preds):
+                node = p.node
+                if prog == "edges":          # <<A>>_v = A /\ ~UNCHANGED v
+                    a, sub = node.a
+                    node = Node("and", ((a, Node("not", (Node("unchanged", (sub,)),))),), node.line, node.col)
+                ok, bad = Label("lok"), Label("lbad")
+                mk = self.mark()
+                self.bound = bound
+                self.cc(node, _label_env(p.env), p.ctx, "N", ok, bad)
+                self.release(mk)
+                self.asm.label(bad)
+                self.asm.emit("INVF", j)
+                self.asm.label(ok)
+            self.asm.emit("HALT")
+        for buf in self.sub_bufs:
+            self.asm.splice(buf)
+        code, cpool, ent = self.asm.assemble(entries)
+        img = LabelImage()
+        img.code, img.cpool, img.entries = code, cpool, ent
+        img.frame_words = self.high + 4
+        img.n_states, img.n_edges = len(state_preds), len(edge_preds)
+        limit = frame_class(cm.frame_words)
+        if img.frame_words > limit:
+            raise CompileError(f"the liveness labels need a frame of {img.frame_words} words, more than the "
+                               f"{limit} words the model's kernels have")
+        return img
+
     def _packed_layout(self):
         """Pack order: (frame offset, bit width, bias) per scalar slot."""
         lay = []
@@ -4521,3 +4566,40 @@ class Lowering:
                 return i
         self.actions.append(key)
         return len(self.actions) - 1
+
+
+class LabelImage:
+    """The bytecode of the state-graph labels (DESIGN.md §7h), an image of its own over a model's frame: the program at
+    entries["states"] runs on one stored state (current frame) and the one at entries["edges"] on an edge (s in the
+    current frame, t in the primed one).  Predicate j of a program that is false raises INVF j."""
+
+    def __init__(self):
+        self.code = None
+        self.cpool = None
+        self.entries = {}
+        self.frame_words = 0
+        self.n_states = 0
+        self.n_edges = 0
+
+
+def frame_class(words):
+    """The frame the interpreter kernels give a model of `words` frame words (vm_frame_class in csrc/tlag_engine.cu)"""
+    c = 64
+    while c < 8192 and c < words:
+        c *= 2
+    return c
+
+
+def compile_labels(m, cm: CompiledModel, state_preds, edge_preds) -> LabelImage:
+    """Lower the state predicates and the actions <<A>>_v (front/spec.py Pred) of model m into a label image over cm's
+    layout, atom table and frame; cm itself is not touched.  An image that needs more than the frame the model's
+    kernels have (frame_class) is a CompileError."""
+    lw = Lowering(m, seq_cap=cm.seq_cap)
+    lw.atoms, lw.codec = cm.atoms, cm.codec
+    lw.var_types = cm.var_types
+    lw.group = []
+    return lw._compile_labels(cm, state_preds, edge_preds)
+
+
+def _label_env(env):
+    return {k: Const(v) for k, v in env.items()}

@@ -124,6 +124,8 @@ struct tlag_engine {
   unsigned long long* d_goff = nullptr; uint32_t* d_gdst = nullptr; uint32_t* d_gact = nullptr;
   uint64_t g_cap = 0, g_edges = 0, g_states = 0, g_expanded = 0; bool g_ready = false;
   uint64_t graph_edges = 1ULL << 24;  // edges the chunk buffer of the edge pass starts with (TLAG_GRAPH_EDGES: test hook)
+  // the graph's liveness labels (tlag_label_graph): one word per row and one per edge, released with the graph
+  uint32_t* d_slab = nullptr; uint32_t* d_elab = nullptr;
 };
 
 // ------------------------------------------------------------------ sliced native build
@@ -600,6 +602,91 @@ __global__ void k_fill_u64(unsigned long long* __restrict__ a, unsigned long lon
   if (i < n) a[i] = v;
 }
 
+// ---- liveness labels (include/tlag.h: tlag_label_graph)
+struct LabelParams {
+  const uint64_t* code; const int32_t* cpool;   // the label image
+  uint32_t entry;                                // its state or edge program
+  uint32_t all;                                  // the program's bits
+  const unsigned long long* off; const uint32_t* dst;   // the resident CSR (edge labels)
+  unsigned long long n;                          // lanes: rows (state labels) or edges
+  unsigned long long rows;                       // rows of the CSR
+  uint32_t* out;                                 // one word per lane: bit j = predicate j holds
+  unsigned long long* bad;                       // a predicate trapped
+};
+
+// One lane per stored row (EDGES false) or per edge of the resident CSR (EDGES true: its source row unpacked to the current
+// frame, its destination to the primed one), on the warp-scheduled interpreter of k_wave.  The program raises INVF j for
+// each predicate j that is false; the lane's word gets the others.
+template <int FRAME, bool EDGES>
+__global__ void __launch_bounds__(TLAG_BLOCK, TLAG_WAVE_OCC(FRAME, false))
+k_label(DevParams p, LabelParams l) {
+  int32_t frame[FRAME];
+  uint32_t w[TLAG_MAXW];
+  const unsigned lane = threadIdx.x & 31;
+  const int W = p.W;
+  const unsigned long long stride = (unsigned long long)gridDim.x * blockDim.x;
+  for (unsigned long long base = (unsigned long long)blockIdx.x * blockDim.x + (threadIdx.x & ~31u); base < l.n;
+       base += stride) {
+    const unsigned long long i = base + lane;
+    const bool active = i < l.n;
+    if (active) {
+      unsigned long long s = i;
+      if (EDGES) {                       // the row whose edges hold edge i: the last s with off[s] <= i
+        unsigned long long lo = 0, hi = l.rows - 1;
+        while (lo < hi) {
+          const unsigned long long mid = (lo + hi + 1) >> 1;
+          if (l.off[mid] <= i) lo = mid; else hi = mid - 1;
+        }
+        s = lo;
+      }
+      vm_load_row(p, W, s, w, frame);
+      if (EDGES) {
+        const uint32_t* t = p.states + (unsigned long long)l.dst[i] * W;
+        for (int k = 0; k < W; ++k) w[k] = t[k];
+        tlag_unpack(p.layout, p.n_slots, w, frame + p.p_off);
+      }
+    }
+    uint32_t fails = 0;
+    int ev = 0;
+    int32_t info = 0, info2 = 0;
+    bool run = active;
+    uint32_t pc = active ? l.entry : TLAG_PC_PARKED, rpc = 0;
+    for (;;) {
+      warp_vm<false, false>(l.code, nullptr, l.cpool, frame, pc, rpc, ev, info, info2);
+      if (run) {
+        if (ev == TLAG_EV_INVF) {
+          fails |= 1u << (info & 31);
+          pc = rpc;
+        } else {
+          if (ev != TLAG_EV_HALT) atomicExch(l.bad, 1ULL);
+          run = false;
+        }
+      }
+      if (!__any_sync(0xffffffffu, pc != TLAG_PC_PARKED)) break;
+    }
+    if (active) l.out[i] = ~fails & l.all;
+  }
+}
+
+// state bits derived from each row's out-edges: en[b] (< 32) is set when some edge has edge bit b (ENABLED <<A_b>>_v),
+// nen[b] when none has
+struct EnabledMap { uint8_t en[32], nen[32]; };
+
+__global__ void k_label_enabled(const unsigned long long* __restrict__ off, const uint32_t* __restrict__ elab,
+                                unsigned long long n, EnabledMap m, uint32_t* __restrict__ slab) {
+  for (unsigned long long s = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; s < n;
+       s += (unsigned long long)gridDim.x * blockDim.x) {
+    uint32_t x = 0;
+    for (unsigned long long j = off[s], e = off[s + 1]; j < e; ++j) x |= elab[j];
+    uint32_t word = slab[s];
+    for (int b = 0; b < 32; ++b) {
+      if (m.en[b] < 32 && ((x >> b) & 1u)) word |= 1u << m.en[b];
+      if (m.nen[b] < 32 && !((x >> b) & 1u)) word |= 1u << m.nen[b];
+    }
+    slab[s] = word;
+  }
+}
+
 // XOR and SUM of tlag_edge_term over the edges out of rows [0, n)
 __global__ void k_graph_digest(DevParams p, const unsigned long long* __restrict__ off, const uint32_t* __restrict__ dst,
                                const uint32_t* __restrict__ act, unsigned long long n, unsigned long long* out2) {
@@ -1005,10 +1092,10 @@ static cudaError_t allow_smem(K fn, size_t bytes) {
 static inline size_t vm_smem(const tlag_engine* e) { return e->p.code_in_smem ? (size_t)e->p.code_len * 8 : 0; }
 
 // Interpreter kernel fn over `rows` rows, one lane per row (k_wave: a warp per 32-row chunk, the same count), on a
-// persistent grid: at most one resident wave of CTAs, at least one CTA
+// persistent grid: at most one resident wave of CTAs, at least one CTA.  launch_vm gives it the engine's program in
+// shared memory when the engine's variant runs it from there; launch_vm_smem takes the size
 template <class... P, class... A>
-static cudaError_t launch_vm(tlag_engine* e, void (*fn)(P...), uint64_t rows, const A&... args) {
-  const size_t smem = vm_smem(e);
+static cudaError_t launch_vm_smem(tlag_engine* e, size_t smem, void (*fn)(P...), uint64_t rows, const A&... args) {
   const cudaError_t r = allow_smem(fn, smem);
   if (r != cudaSuccess) return r;
   int occ = 1;
@@ -1019,6 +1106,10 @@ static cudaError_t launch_vm(tlag_engine* e, void (*fn)(P...), uint64_t rows, co
   fn<<<(unsigned)blocks, TLAG_BLOCK, smem, e->stream>>>(args...);
   e->launches++;
   return cudaGetLastError();
+}
+template <class... P, class... A>
+static cudaError_t launch_vm(tlag_engine* e, void (*fn)(P...), uint64_t rows, const A&... args) {
+  return launch_vm_smem(e, vm_smem(e), fn, rows, args...);
 }
 
 // The engine's variant of an interpreter kernel template: its frame class, the program in shared memory or not, and up to
@@ -1456,8 +1547,8 @@ static void read_env_hooks(tlag_engine* e) {
 
 // The state graph is a picture of the store after a search call: any call that changes the store drops it.
 static void release_graph(tlag_engine* e) {
-  dfree(e, e->d_goff); dfree(e, e->d_gdst); dfree(e, e->d_gact);
-  e->d_goff = nullptr; e->d_gdst = e->d_gact = nullptr;
+  dfree(e, e->d_goff); dfree(e, e->d_gdst); dfree(e, e->d_gact); dfree(e, e->d_slab); dfree(e, e->d_elab);
+  e->d_goff = nullptr; e->d_gdst = e->d_gact = nullptr; e->d_slab = e->d_elab = nullptr;
   e->g_cap = e->g_edges = e->g_states = e->g_expanded = 0;
   e->g_ready = false;
 }
@@ -2680,4 +2771,99 @@ extern "C" int tlag_graph_digest(tlag_engine* e, uint64_t* xor_out, uint64_t* su
     return TLAG_OK;
   });
 #endif
+}
+
+// ---- liveness labels (include/tlag.h: tlag_label_graph, tlag_graph_view) -------------------------------------------------
+#if !defined(TLAG_SL_SIM)
+template <bool EDGES>
+static cudaError_t launch_label(tlag_engine* e, const LabelParams& l) {
+#if defined(TLAG_SLICED_INC)   // the one frame class of the library's model, as its k_graph
+  const auto fn = k_label<vm_frame_class(TLAG_SL_FRAME), EDGES>;
+#else
+  const auto fn = vm_variant(e, [](auto f, auto, auto) { return k_label<f, EDGES>; });
+#endif
+  return launch_vm_smem(e, 0, fn, l.n, e->p, l);
+}
+#endif
+
+extern "C" int tlag_label_graph(tlag_engine* e, const tlag_label_program* lp, float* device_ms) {
+  if (!e || !lp) return TLAG_EINVAL;
+#if defined(TLAG_SL_SIM)
+  e->err = "this library holds the model's simulation kernels only";
+  return TLAG_EINVAL;
+#else
+  if (!e->g_ready) { e->err = "no state graph: tlag_build_graph first"; return TLAG_ESTATE; }
+  if (!lp->code || !lp->code_len || lp->entry_states >= lp->code_len || lp->entry_edges >= lp->code_len ||
+      lp->n_state_preds > 32 || lp->n_edge_preds > 32 || (lp->cpool_len && !lp->cpool)) {
+    e->err = "tlag_label_graph: missing program, an entry outside it, or more than 32 state or edge predicates";
+    return TLAG_EINVAL;
+  }
+  EnabledMap em;
+  for (int b = 0; b < 32; ++b) {
+    em.en[b] = lp->en_bit[b]; em.nen[b] = lp->nen_bit[b];
+    if ((em.en[b] < 32 || em.nen[b] < 32) && (uint32_t)b >= lp->n_edge_preds) {
+      e->err = "tlag_label_graph: an ENABLED bit of an edge predicate the program does not have";
+      return TLAG_EINVAL;
+    }
+    if ((em.en[b] != 0xFF && em.en[b] >= 32) || (em.nen[b] != 0xFF && em.nen[b] >= 32)) {
+      e->err = "tlag_label_graph: an ENABLED bit past bit 31";
+      return TLAG_EINVAL;
+    }
+  }
+  dfree(e, e->d_slab); dfree(e, e->d_elab);
+  e->d_slab = e->d_elab = nullptr;
+  uint64_t* code = nullptr; int32_t* cpool = nullptr; unsigned long long* bad = nullptr;
+  if (dmalloc(e, &e->d_slab, (e->g_states ? e->g_states : 1) * 4) != cudaSuccess ||
+      dmalloc(e, &e->d_elab, (e->g_edges ? e->g_edges : 1) * 4) != cudaSuccess ||
+      dmalloc(e, &code, (uint64_t)lp->code_len * 8) != cudaSuccess ||
+      dmalloc(e, &cpool, (uint64_t)(lp->cpool_len ? lp->cpool_len : 1) * 4) != cudaSuccess ||
+      dmalloc(e, &bad, 8) != cudaSuccess) {
+    cudaGetLastError();
+    dfree(e, code); dfree(e, cpool); dfree(e, bad);
+    dfree(e, e->d_slab); dfree(e, e->d_elab);
+    e->d_slab = e->d_elab = nullptr;
+    e->err = "tlag_label_graph: not enough device memory for the labels";
+    return TLAG_ENOMEM;
+  }
+  float ms = 0;
+  unsigned long long hbad = 0;
+  int r = timed(e, &ms, nullptr, [&] {
+    CK(cudaMemcpyAsync(code, lp->code, (uint64_t)lp->code_len * 8, cudaMemcpyHostToDevice, e->stream));
+    if (lp->cpool_len) CK(cudaMemcpyAsync(cpool, lp->cpool, (uint64_t)lp->cpool_len * 4, cudaMemcpyHostToDevice, e->stream));
+    CK(cudaMemsetAsync(bad, 0, 8, e->stream));
+    LabelParams l;
+    l.code = code; l.cpool = cpool; l.off = e->d_goff; l.dst = e->d_gdst; l.rows = e->g_states; l.bad = bad;
+    l.entry = lp->entry_states; l.all = lp->n_state_preds == 32 ? 0xFFFFFFFFu : (1u << lp->n_state_preds) - 1;
+    l.n = e->g_states; l.out = e->d_slab;
+    if (l.n) CK(launch_label<false>(e, l));
+    l.entry = lp->entry_edges; l.all = lp->n_edge_preds == 32 ? 0xFFFFFFFFu : (1u << lp->n_edge_preds) - 1;
+    l.n = e->g_edges; l.out = e->d_elab;
+    if (l.n) CK(launch_label<true>(e, l));
+    if (e->g_states) {
+      k_label_enabled<<<e->sm_count * 8, 256, 0, e->stream>>>(e->d_goff, e->d_elab, e->g_states, em, e->d_slab);
+      e->launches++;
+      CK(cudaGetLastError());
+    }
+    CK(cudaMemcpyAsync(&hbad, bad, 8, cudaMemcpyDeviceToHost, e->stream));
+    return TLAG_OK;
+  });
+  dfree(e, code); dfree(e, cpool); dfree(e, bad);
+  if (!r) CK(cudaStreamSynchronize(e->stream));
+  if (!r && hbad) { e->err = "tlag_label_graph: a label predicate trapped (it cannot be evaluated on some state or edge)"; r = TLAG_EEVAL; }
+  if (r) { dfree(e, e->d_slab); dfree(e, e->d_elab); e->d_slab = e->d_elab = nullptr; return r; }
+  if (device_ms) *device_ms = ms;
+  return TLAG_OK;
+#endif
+}
+
+extern "C" int tlag_graph_view(tlag_engine* e, tlag_graph_dev* out) {
+  if (!e || !out) return TLAG_EINVAL;
+  memset(out, 0, sizeof(*out));
+  if (!e->g_ready) { e->err = "no state graph: tlag_build_graph first"; return TLAG_ESTATE; }
+  CK(cudaStreamSynchronize(e->stream));
+  out->n_states = e->g_states; out->n_edges = e->g_edges; out->n_init = e->init_states;
+  out->off = (uint64_t)(uintptr_t)e->d_goff; out->dst = (uint64_t)(uintptr_t)e->d_gdst;
+  out->state_label = (uint64_t)(uintptr_t)e->d_slab; out->edge_label = (uint64_t)(uintptr_t)e->d_elab;
+  out->device = e->m.device;
+  return TLAG_OK;
 }

@@ -35,7 +35,10 @@ thread_local std::string g_err;
     cudaError_t _e = (call);                                                             \
     if (_e != cudaSuccess) {                                                             \
       g_err = std::string(#call) + ": " + cudaGetErrorString(_e);                        \
-      return TLAG_ECUDA;                                                                 \
+      if (_e != cudaErrorMemoryAllocation) return TLAG_ECUDA;                            \
+      cudaGetLastError();                                                                \
+      g_err += " (the graph does not fit in device memory)";                             \
+      return TLAG_ENOMEM;                                                                \
     }                                                                                    \
   } while (0)
 #define GR(call)                                                                         \
@@ -260,6 +263,90 @@ __global__ void k_count_roots(uint32_t n, const uint32_t* scc, unsigned int* cnt
   GRID_STRIDE(v, n) if (scc[v] == (uint32_t)v) atomicAdd(cnt, 1u);
 }
 
+// ---- the engine's labelled graph (tlag_live_check)
+// the source row of every CSR edge
+__global__ void k_csr_src(uint32_t n, const u64* off, uint32_t* src) {
+  GRID_STRIDE(v, n) for (u64 j = off[v], e = off[v + 1]; j < e; ++j) src[j] = (uint32_t)v;
+}
+
+// the restriction and the seeds from the label words
+__global__ void k_live_masks(uint32_t n, const uint32_t* slab, uint32_t keep_set, uint32_t keep_clear, uint32_t seed_set,
+                             uint32_t seed_clear, uint64_t seed_rows, uint8_t* vmask, uint8_t* seeds) {
+  GRID_STRIDE(v, n) {
+    const uint32_t x = slab[v];
+    vmask[v] = (x & keep_set) == keep_set && !(x & keep_clear);
+    seeds[v] = v < seed_rows && (x & seed_set) == seed_set && !(x & seed_clear);
+  }
+}
+
+__global__ void k_edge_drop(uint64_t m, const uint32_t* elab, uint32_t drop, uint8_t* em) {
+  GRID_STRIDE(i, m) em[i] = !(elab[i] & drop);
+}
+
+__global__ void k_first_seed(uint32_t n, const uint8_t* seeds, unsigned int* first) {
+  GRID_STRIDE(v, n) if (seeds[v]) atomicMin(first, (unsigned)v);
+}
+
+// ---- lasso: breadth-first search with parent pointers inside `allowed`, from the vertices with par[v] == v
+__global__ void k_bfs_init(uint32_t n, const uint8_t* src, uint32_t one, uint32_t* par, uint8_t* cur) {
+  GRID_STRIDE(v, n) {
+    const bool s = src ? src[v] != 0 : (uint32_t)v == one;
+    par[v] = s ? (uint32_t)v : kOut;
+    cur[v] = s;
+  }
+}
+
+__global__ void k_bfs_step(uint32_t n, const uint32_t* off, const uint32_t* adj, const uint8_t* allowed, uint32_t* par,
+                           const uint8_t* cur, uint8_t* nxt, const uint8_t* target, unsigned int* flag) {
+  GRID_STRIDE(v, n) {
+    if (!cur[v]) continue;
+    for (uint32_t j = off[v], e = off[v + 1]; j < e; ++j) {
+      const uint32_t w = adj[j];
+      if (!allowed[w] || par[w] != kOut) continue;
+      if (atomicCAS(&par[w], kOut, (uint32_t)v) == kOut) {
+        nxt[w] = 1;
+        flag[0] = 1;
+        if (target[w]) atomicMin(&flag[1], w);
+      }
+    }
+  }
+}
+
+__global__ void k_bfs_hit(uint32_t n, const uint8_t* cur, const uint8_t* target, unsigned int* flag) {
+  GRID_STRIDE(v, n) if (cur[v] && target[v]) atomicMin(&flag[1], (unsigned)v);
+}
+
+// targets inside SCC c: the states with a `clear` bit clear (clear != 0), or the sources of the SCC's edges with an
+// `act` bit, next[source] = the edge's destination
+__global__ void k_scc_targets(uint32_t n, uint32_t m, const uint32_t* res, uint32_t c, const uint32_t* word, uint32_t clear,
+                              const uint32_t* src, const uint32_t* dst, const uint32_t* lab, uint32_t act, uint8_t* target,
+                              uint32_t* next) {
+  GRID_STRIDE(i, (uint64_t)n > m ? n : m) {
+    if (clear && i < n) target[i] = res[i] == c && (~word[i] & clear) != 0;
+    if (act && i < m && res[src[i]] == c && res[dst[i]] == c && (lab[i] & act)) {
+      target[src[i]] = 1;
+      next[src[i]] = dst[i];
+    }
+  }
+}
+
+// the path from v back along par[] to its root (par[root] == root), v first: out[0, min(len, cap)), *len
+__global__ void k_walk_parents(const uint32_t* par, uint32_t v, uint32_t cap, uint32_t* out, unsigned int* len) {
+  uint32_t k = 0;
+  for (;;) {
+    if (k < cap) out[k] = v;
+    ++k;
+    const uint32_t p = par[v];
+    if (p == v || k > cap) break;
+    v = p;
+  }
+  *len = k;
+}
+
+__global__ void k_in_scc(uint32_t n, const uint32_t* res, uint32_t c, uint8_t* in) {
+  GRID_STRIDE(v, n) in[v] = res[v] == c;
+}
+
 template <class T>
 struct DevBuf {
   T* p = nullptr;
@@ -310,23 +397,34 @@ struct Graph {
     return TLAG_OK;
   }
 
-  int upload(const tlag_graph* g) {
-    if (!g || !g->src || !g->dst || g->n_states >= kActive || g->n_edges >= 0xFFFFFFFFull) {
-      g_err = "tlag_graph: missing edge arrays, or n_states >= 2^32 - 2 or n_edges >= 2^32 - 1";
+  // the stream, events and flags on the graph's device, for n_states states and n_edges edges
+  int init(uint64_t n_states, uint64_t n_edges, int device, const char* what) {
+    if (n_states >= kActive || n_edges >= 0xFFFFFFFFull) {
+      g_err = std::string(what) + ": n_states >= 2^32 - 2 or n_edges >= 2^32 - 1";
       return TLAG_EINVAL;
     }
-    n = (uint32_t)g->n_states;
-    GK(cudaSetDevice(g->device));
+    n = (uint32_t)n_states;
+    GK(cudaSetDevice(device));
     int sms = 0;
-    GK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, g->device));
+    GK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
     grid = sms * 8;
     GK(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
     GK(cudaEventCreate(&ev0));
     GK(cudaEventCreate(&ev1));
     GK(cudaMallocHost((void**)&h_flag, 2 * sizeof(unsigned int)));
     GK(flag.alloc(2));
+    GK(vmask.alloc(n)); GK(alive.alloc(n)); GK(word.alloc(n));
+    return TLAG_OK;
+  }
+
+  // a host edge list: copied to the device, then build()
+  int upload(const tlag_graph* g) {
+    if (!g || !g->src || !g->dst) {
+      g_err = "tlag_graph: missing edge arrays";
+      return TLAG_EINVAL;
+    }
+    GR(init(g->n_states, g->n_edges, g->device, "tlag_graph"));
     uint64_t m0 = g->n_edges;
-    // raw edge list -> compacted (src, dst, label)
     DevBuf<uint32_t> rs, rd, rl;
     DevBuf<uint8_t> em;
     GK(rs.alloc(m0)); GK(rd.alloc(m0));
@@ -340,18 +438,22 @@ struct Graph {
       GK(em.alloc(m0));
       GK(cudaMemcpyAsync(em.p, g->edge_mask, m0, cudaMemcpyHostToDevice, st));
     }
-    GK(vmask.alloc(n)); GK(alive.alloc(n));
     if (g->state_mask) GK(cudaMemcpyAsync(vmask.p, g->state_mask, n, cudaMemcpyHostToDevice, st));
     else GK(cudaMemsetAsync(vmask.p, 1, n, st));
-    GK(cudaMemcpyAsync(alive.p, vmask.p, n, cudaMemcpyDeviceToDevice, st));
-    GK(word.alloc(n));
     if (g->state_label) GK(cudaMemcpyAsync(word.p, g->state_label, (uint64_t)n * 4, cudaMemcpyHostToDevice, st));
     else GK(cudaMemsetAsync(word.p, 0, (uint64_t)n * 4, st));
-    GK(src.alloc(m0)); GK(dst.alloc(m0)); GK(lab.alloc(m0));
     GK(cudaEventRecord(ev0, st));
+    return build(rs, rd, rl.p, em.p, m0);
+  }
+
+  // device compaction and both CSRs: the edges (rs, rd; labels rl, mask em may be null) of m0 edges, vmask and word set;
+  // rs and rd are the sorts' scratch afterwards
+  int build(DevBuf<uint32_t>& rs, DevBuf<uint32_t>& rd, const uint32_t* rl, const uint8_t* em, uint64_t m0) {
+    GK(cudaMemcpyAsync(alive.p, vmask.p, n, cudaMemcpyDeviceToDevice, st));
+    GK(src.alloc(m0)); GK(dst.alloc(m0)); GK(lab.alloc(m0));
     GK(cudaMemsetAsync(flag.p, 0, 2 * sizeof(unsigned int), st));
     if (m0)
-      k_keep_edges<<<grid_for(m0), kBlock, 0, st>>>(n, m0, rs.p, rd.p, rl.p, em.p, vmask.p, src.p, dst.p, lab.p, flag.p);
+      k_keep_edges<<<grid_for(m0), kBlock, 0, st>>>(n, m0, rs.p, rd.p, rl, em, vmask.p, src.p, dst.p, lab.p, flag.p);
     GK(cudaGetLastError());
     GK(cudaMemcpyAsync(h_flag, flag.p, 2 * sizeof(unsigned int), cudaMemcpyDeviceToHost, st));
     GK(cudaStreamSynchronize(st));
@@ -463,6 +565,53 @@ struct Graph {
   }
 };
 
+
+// The Emerson-Lei search of tlag_fair_cycles and tlag_live_check on a built Graph: decompose, drop what fails, decompose
+// again while an SF test split an SCC; then the accepted SCCs reachable from the seeds (device flags, or all).
+// res[v] = accepted SCC id of v or kOut; s_or / s_and / e_or: the last decomposition's aggregates, exact for accepted SCCs.
+struct FairSearch {
+  DevBuf<uint32_t> s_or, s_and, e_or, res;
+  DevBuf<unsigned int> cnt;     // {witness, accepted SCCs}
+  unsigned int h_cnt[2] = {kOut, 0};
+  uint32_t rounds = 0;
+  const u64* reach = nullptr;   // G.b: reachable from the seeds (null: no seeds)
+
+  int run(Graph& G, const FairSet& fs, const uint8_t* seeds) {
+    const uint32_t n = G.n;
+    GK(s_or.alloc(n)); GK(s_and.alloc(n)); GK(e_or.alloc(n)); GK(res.alloc(n));
+    for (;;) {
+      ++rounds;
+      GR(G.decompose());
+      if (!n) break;
+      GK(cudaMemsetAsync(s_or.p, 0, (uint64_t)n * 4, G.st));
+      GK(cudaMemsetAsync(s_and.p, 0xFF, (uint64_t)n * 4, G.st));
+      GK(cudaMemsetAsync(e_or.p, 0, (uint64_t)n * 4, G.st));
+      k_state_agg<<<G.grid_for(n), kBlock, 0, G.st>>>(n, G.scc.p, G.word.p, s_or.p, s_and.p);
+      if (G.m) k_edge_agg<<<G.grid_for(G.m), kBlock, 0, G.st>>>(G.m, G.src.p, G.dst.p, G.lab.p, G.scc.p, e_or.p);
+      GR(G.clear_flag());
+      k_judge<<<G.grid_for(n), kBlock, 0, G.st>>>(n, G.scc.p, G.word.p, s_or.p, s_and.p, e_or.p, fs, G.alive.p, G.flag.p);
+      GK(cudaGetLastError());
+      unsigned int resplit = 0;
+      GR(G.read_flag(&resplit));
+      if (!resplit) break;
+    }
+    // reachability from the seeds over the whole restricted graph (every compacted edge), into b[]
+    GK(cnt.alloc(2));
+    GK(cudaMemcpyAsync(cnt.p, h_cnt, sizeof h_cnt, cudaMemcpyHostToDevice, G.st));
+    if (seeds && n) {
+      k_reach_seed<<<G.grid_for(n), kBlock, 0, G.st>>>(n, seeds, G.vmask.p, G.b.p, G.cur.p);
+      GK(cudaGetLastError());
+      GR(G.propagate(G.foff.p, G.fadj.p, G.b.p, nullptr, nullptr));
+      reach = G.b.p;
+    }
+    if (n) k_result<<<G.grid_for(n), kBlock, 0, G.st>>>(n, G.scc.p, G.alive.p, reach, res.p, cnt.p, cnt.p + 1);
+    GK(cudaGetLastError());
+    GK(cudaMemcpyAsync(h_cnt, cnt.p, sizeof h_cnt, cudaMemcpyDeviceToHost, G.st));
+    GK(cudaStreamSynchronize(G.st));
+    return TLAG_OK;
+  }
+};
+
 }  // namespace
 
 extern "C" const char* tlag_graph_last_error(void) { return g_err.c_str(); }
@@ -486,77 +635,230 @@ extern "C" int tlag_scc(const tlag_graph* g, uint32_t* scc_out, uint64_t* n_scc_
   return TLAG_OK;
 }
 
-extern "C" int tlag_fair_cycles(const tlag_graph* g, const tlag_fair_query* q, uint32_t* scc_out, tlag_fair_result* out) {
-  g_err.clear();
-  if (!q || !out || (q->n_fair && !q->fair) || q->n_fair > 64) {
-    g_err = "tlag_fair_cycles: missing query or result, or more than 64 fairness conditions";
+// the conditions of a query, WF first, then SF
+static int fair_set(const tlag_fairness* fair, uint32_t n_fair, uint32_t need_clear, FairSet* fs, const char* what) {
+  if ((n_fair && !fair) || n_fair > 64) {
+    g_err = std::string(what) + ": missing fairness conditions, or more than 64";
     return TLAG_EINVAL;
   }
-  FairSet fs;
-  memset(&fs, 0, sizeof fs);
-  fs.need_clear = q->need_clear;
+  memset(fs, 0, sizeof *fs);
+  fs->need_clear = need_clear;
   for (int kind = TLAG_FAIR_WF; kind <= TLAG_FAIR_SF; ++kind)
-    for (uint32_t k = 0; k < q->n_fair; ++k) {
-      const tlag_fairness& f = q->fair[k];
+    for (uint32_t k = 0; k < n_fair; ++k) {
+      const tlag_fairness& f = fair[k];
       if (f.kind > TLAG_FAIR_SF || f.enabled_bit > 31 || f.action_bit > 31) {
-        g_err = "tlag_fair_cycles: fairness condition " + std::to_string(k) + " has a bad kind or bit";
+        g_err = std::string(what) + ": fairness condition " + std::to_string(k) + " has a bad kind or bit";
         return TLAG_EINVAL;
       }
       if ((int)f.kind != kind) continue;
-      uint32_t at = fs.n_wf + fs.n_sf;
-      fs.en[at] = 1u << f.enabled_bit;
-      fs.act[at] = 1u << f.action_bit;
-      if (kind == TLAG_FAIR_WF) ++fs.n_wf; else ++fs.n_sf;
+      uint32_t at = fs->n_wf + fs->n_sf;
+      fs->en[at] = 1u << f.enabled_bit;
+      fs->act[at] = 1u << f.action_bit;
+      if (kind == TLAG_FAIR_WF) ++fs->n_wf; else ++fs->n_sf;
     }
+  return TLAG_OK;
+}
+
+extern "C" int tlag_fair_cycles(const tlag_graph* g, const tlag_fair_query* q, uint32_t* scc_out, tlag_fair_result* out) {
+  g_err.clear();
+  if (!q || !out) {
+    g_err = "tlag_fair_cycles: missing query or result";
+    return TLAG_EINVAL;
+  }
+  FairSet fs;
+  GR(fair_set(q->fair, q->n_fair, q->need_clear, &fs, "tlag_fair_cycles"));
   DeviceGuard dg;
   Graph G;
   GR(G.upload(g));
   const uint32_t n = G.n;
-  DevBuf<uint32_t> s_or, s_and, e_or, res;
-  GK(s_or.alloc(n)); GK(s_and.alloc(n)); GK(e_or.alloc(n)); GK(res.alloc(n));
-  uint32_t rounds = 0;
-  for (;;) {   // Emerson-Lei: decompose, drop what fails, decompose again while an SF test split an SCC
-    ++rounds;
-    GR(G.decompose());
-    if (!n) break;
-    GK(cudaMemsetAsync(s_or.p, 0, (uint64_t)n * 4, G.st));
-    GK(cudaMemsetAsync(s_and.p, 0xFF, (uint64_t)n * 4, G.st));
-    GK(cudaMemsetAsync(e_or.p, 0, (uint64_t)n * 4, G.st));
-    k_state_agg<<<G.grid_for(n), kBlock, 0, G.st>>>(n, G.scc.p, G.word.p, s_or.p, s_and.p);
-    if (G.m) k_edge_agg<<<G.grid_for(G.m), kBlock, 0, G.st>>>(G.m, G.src.p, G.dst.p, G.lab.p, G.scc.p, e_or.p);
-    GR(G.clear_flag());
-    k_judge<<<G.grid_for(n), kBlock, 0, G.st>>>(n, G.scc.p, G.word.p, s_or.p, s_and.p, e_or.p, fs, G.alive.p, G.flag.p);
-    GK(cudaGetLastError());
-    unsigned int resplit = 0;
-    GR(G.read_flag(&resplit));
-    if (!resplit) break;
-  }
-  // reachability from the seeds over the whole restricted graph (every compacted edge), into b[]
-  DevBuf<unsigned int> cnt;   // {witness, accepted SCCs}
-  GK(cnt.alloc(2));
-  const unsigned int init_cnt[2] = {kOut, 0};
-  GK(cudaMemcpyAsync(cnt.p, init_cnt, sizeof init_cnt, cudaMemcpyHostToDevice, G.st));
-  const u64* reach = nullptr;
+  FairSearch F;
+  DevBuf<uint8_t> sd;
   if (q->seeds && n) {
-    DevBuf<uint8_t> sd;
     GK(sd.alloc(n));
     GK(cudaMemcpyAsync(sd.p, q->seeds, n, cudaMemcpyHostToDevice, G.st));
-    k_reach_seed<<<G.grid_for(n), kBlock, 0, G.st>>>(n, sd.p, G.vmask.p, G.b.p, G.cur.p);
-    GK(cudaGetLastError());
-    GR(G.propagate(G.foff.p, G.fadj.p, G.b.p, nullptr, nullptr));
-    reach = G.b.p;
   }
-  if (n) k_result<<<G.grid_for(n), kBlock, 0, G.st>>>(n, G.scc.p, G.alive.p, reach, res.p, cnt.p, cnt.p + 1);
-  GK(cudaGetLastError());
+  GR(F.run(G, fs, q->seeds ? sd.p : nullptr));
   float ms = 0;
   GR(G.elapsed(&ms));
-  unsigned int h_cnt[2];
-  GK(cudaMemcpy(h_cnt, cnt.p, sizeof h_cnt, cudaMemcpyDeviceToHost));
-  if (scc_out && n) GK(cudaMemcpy(scc_out, res.p, (uint64_t)n * 4, cudaMemcpyDeviceToHost));
-  out->violated = h_cnt[0] != kOut;
-  out->witness = h_cnt[0];
-  out->fair_sccs = h_cnt[1];
-  out->rounds = rounds;
+  if (scc_out && n) GK(cudaMemcpy(scc_out, F.res.p, (uint64_t)n * 4, cudaMemcpyDeviceToHost));
+  out->violated = F.h_cnt[0] != kOut;
+  out->witness = F.h_cnt[0];
+  out->fair_sccs = F.h_cnt[1];
+  out->rounds = F.rounds;
   out->device_ms = ms;
+  return TLAG_OK;
+}
+
+namespace {
+
+// A shortest path inside `allowed` from the sources (flags src, or the vertex one) to a vertex with target[v] != 0, the
+// source first and the target last, appended to path; the search and the path are the graph's forward CSR.
+int bfs_path(Graph& G, const uint8_t* src, uint32_t one, const uint8_t* allowed, const uint8_t* target, uint32_t* par,
+             uint32_t* walk, std::vector<uint32_t>& path) {
+  const uint32_t n = G.n;
+  k_bfs_init<<<G.grid_for(n), kBlock, 0, G.st>>>(n, src, one, par, G.cur.p);
+  const unsigned int init[2] = {0, kOut};
+  GK(cudaMemcpyAsync(G.flag.p, init, sizeof init, cudaMemcpyHostToDevice, G.st));
+  k_bfs_hit<<<G.grid_for(n), kBlock, 0, G.st>>>(n, G.cur.p, target, G.flag.p);
+  GK(cudaGetLastError());
+  uint8_t *c = G.cur.p, *x = G.nxt.p;
+  for (bool first = true;; first = false) {
+    GK(cudaMemcpyAsync(G.h_flag, G.flag.p, 2 * sizeof(unsigned int), cudaMemcpyDeviceToHost, G.st));
+    GK(cudaStreamSynchronize(G.st));
+    if (G.h_flag[1] != kOut) break;
+    if (!first && !G.h_flag[0]) {      // the last step reached no new vertex
+      g_err = "tlag_live_check: the lasso search found no path to its target (internal error)";
+      return TLAG_EINVAL;
+    }
+    GK(cudaMemsetAsync(x, 0, n, G.st));
+    GK(cudaMemsetAsync(G.flag.p, 0, sizeof(unsigned int), G.st));
+    k_bfs_step<<<G.grid_for(n), kBlock, 0, G.st>>>(n, G.foff.p, G.fadj.p, allowed, par, c, x, target, G.flag.p);
+    GK(cudaGetLastError());
+    std::swap(c, x);
+  }
+  // the parent chain from the target, walked on the device and read back in one copy
+  k_walk_parents<<<1, 1, 0, G.st>>>(par, G.h_flag[1], n, walk, G.flag.p);
+  GK(cudaGetLastError());
+  GK(cudaMemcpyAsync(G.h_flag, G.flag.p, sizeof(unsigned int), cudaMemcpyDeviceToHost, G.st));
+  GK(cudaStreamSynchronize(G.st));
+  std::vector<uint32_t> back(G.h_flag[0]);
+  GK(cudaMemcpyAsync(back.data(), walk, back.size() * 4, cudaMemcpyDeviceToHost, G.st));
+  GK(cudaStreamSynchronize(G.st));
+  path.insert(path.end(), back.rbegin(), back.rend());
+  return TLAG_OK;
+}
+
+}  // namespace
+
+extern "C" int tlag_live_check(const tlag_graph_dev* g, const tlag_live_query* q, uint32_t* lasso_out, uint32_t lasso_cap,
+                               tlag_live_result* out) {
+  g_err.clear();
+  if (!g || !q || !out || !g->off || !g->dst || !g->state_label || !g->edge_label) {
+    g_err = "tlag_live_check: missing graph, labels, query or result";
+    return TLAG_EINVAL;
+  }
+  if (g->n_edges >= 0xFFFFFFFFull) {
+    g_err = "tlag_live_check: the graph has 2^32 - 1 edges or more (the SCC core indexes edges with 32 bits)";
+    return TLAG_EINVAL;
+  }
+  memset(out, 0, sizeof *out);
+  FairSet fs;
+  GR(fair_set(q->fair, q->n_fair, q->need_clear, &fs, "tlag_live_check"));
+  const u64* off = (const u64*)(uintptr_t)g->off;
+  const uint32_t* slab = (const uint32_t*)(uintptr_t)g->state_label;
+  const uint32_t* elab = (const uint32_t*)(uintptr_t)g->edge_label;
+  DeviceGuard dg;
+  Graph G;
+  GR(G.init(g->n_states, g->n_edges, g->device, "tlag_live_check"));
+  const uint32_t n = G.n;
+  const uint64_t m0 = g->n_edges;
+  GK(cudaEventRecord(G.ev0, G.st));
+  DevBuf<uint32_t> rs, rd;
+  DevBuf<uint8_t> em, seeds;
+  GK(rs.alloc(m0)); GK(rd.alloc(m0)); GK(em.alloc(m0)); GK(seeds.alloc(n));
+  if (n) {
+    k_csr_src<<<G.grid_for(n), kBlock, 0, G.st>>>(n, off, rs.p);
+    k_live_masks<<<G.grid_for(n), kBlock, 0, G.st>>>(n, slab, q->keep_set, q->keep_clear, q->seed_set, q->seed_clear,
+                                                     q->seed_rows ? q->seed_rows : n, G.vmask.p, seeds.p);
+    GK(cudaMemcpyAsync(G.word.p, slab, (uint64_t)n * 4, cudaMemcpyDeviceToDevice, G.st));
+  }
+  if (m0) {
+    GK(cudaMemcpyAsync(rd.p, (const uint32_t*)(uintptr_t)g->dst, m0 * 4, cudaMemcpyDeviceToDevice, G.st));
+    k_edge_drop<<<G.grid_for(m0), kBlock, 0, G.st>>>(m0, elab, q->edge_drop, em.p);
+  }
+  GK(cudaGetLastError());
+  uint32_t witness = kOut;
+  FairSearch F;
+  if (q->flags & TLAG_LIVE_ANY_SEED) {
+    GK(F.cnt.alloc(2));
+    GK(cudaMemcpyAsync(F.cnt.p, F.h_cnt, sizeof F.h_cnt, cudaMemcpyHostToDevice, G.st));
+    if (n) k_first_seed<<<G.grid_for(n), kBlock, 0, G.st>>>(n, seeds.p, F.cnt.p);
+    GK(cudaGetLastError());
+    GK(cudaMemcpyAsync(F.h_cnt, F.cnt.p, sizeof F.h_cnt, cudaMemcpyDeviceToHost, G.st));
+    GK(cudaStreamSynchronize(G.st));
+    witness = F.h_cnt[0];
+  } else {
+    GR(G.build(rs, rd, elab, em.p, m0));
+    GR(F.run(G, fs, (q->flags & TLAG_LIVE_SEEDS) ? seeds.p : nullptr));
+    witness = F.h_cnt[0];
+    out->fair_sccs = F.h_cnt[1];
+    out->rounds = F.rounds;
+  }
+  GR(G.elapsed(&out->check_ms));
+  out->violated = witness != kOut;
+  out->witness = witness;
+  if (!out->violated || (q->flags & TLAG_LIVE_ANY_SEED)) {
+    if (out->violated) {
+      out->prefix_len = 1;
+      if (lasso_cap < 1) return TLAG_EOVERFLOW;
+      if (lasso_out) lasso_out[0] = witness;
+    }
+    return TLAG_OK;
+  }
+  // the lasso
+  GK(cudaEventRecord(G.ev0, G.st));
+  std::vector<uint32_t> prefix, cycle;
+  DevBuf<uint32_t> par, next, walk;
+  DevBuf<uint8_t> target, inscc;
+  GK(par.alloc(n)); GK(next.alloc(n)); GK(walk.alloc(n)); GK(target.alloc(n)); GK(inscc.alloc(n));
+  if (q->flags & TLAG_LIVE_SEEDS) {   // seed -> witness inside the restriction
+    GK(cudaMemsetAsync(target.p, 0, n, G.st));
+    GK(cudaMemsetAsync(target.p + witness, 1, 1, G.st));
+    GR(bfs_path(G, seeds.p, 0, G.vmask.p, target.p, par.p, walk.p, prefix));
+  } else {
+    prefix.push_back(witness);
+  }
+  uint32_t c = 0, s_and = 0, e_or = 0;
+  GK(cudaMemcpy(&c, F.res.p + witness, 4, cudaMemcpyDeviceToHost));
+  GK(cudaMemcpy(&s_and, F.s_and.p + c, 4, cudaMemcpyDeviceToHost));
+  GK(cudaMemcpy(&e_or, F.e_or.p + c, 4, cudaMemcpyDeviceToHost));
+  k_in_scc<<<G.grid_for(n), kBlock, 0, G.st>>>(n, F.res.p, c, inscc.p);
+  GK(cudaGetLastError());
+  // the cycle's stops: an A-edge of every condition whose action occurs in the SCC, else (WF) a ~EN state; a state with
+  // each need_clear bit clear
+  std::vector<std::pair<uint32_t, uint32_t>> stops;   // (state bits to find clear, edge bits to take)
+  for (uint32_t k = 0; k < fs.n_wf + fs.n_sf; ++k) {
+    if (e_or & fs.act[k]) stops.push_back({0u, fs.act[k]});
+    else if (k < fs.n_wf && (s_and & fs.en[k])) {
+      g_err = "tlag_live_check: an accepted SCC fails a WF condition (internal error)";
+      return TLAG_EINVAL;
+    } else if (k < fs.n_wf) stops.push_back({fs.en[k], 0u});
+  }
+  for (uint32_t b = 0; b < 32; ++b)
+    if (fs.need_clear & (1u << b)) stops.push_back({1u << b, 0u});
+  cycle.push_back(witness);
+  uint32_t at = witness;
+  for (const auto& st : stops) {
+    GK(cudaMemsetAsync(target.p, 0, n, G.st));
+    const uint32_t grid_n = n > G.m ? n : G.m;
+    k_scc_targets<<<G.grid_for(grid_n ? grid_n : 1), kBlock, 0, G.st>>>(n, G.m, F.res.p, c, G.word.p, st.first, G.src.p,
+                                                                        G.dst.p, G.lab.p, st.second, target.p, next.p);
+    GK(cudaGetLastError());
+    std::vector<uint32_t> leg;
+    GR(bfs_path(G, nullptr, at, inscc.p, target.p, par.p, walk.p, leg));
+    cycle.insert(cycle.end(), leg.begin() + 1, leg.end());
+    at = leg.back();
+    if (st.second) {
+      GK(cudaMemcpy(&at, next.p + at, 4, cudaMemcpyDeviceToHost));
+      cycle.push_back(at);
+    }
+  }
+  if (at != witness) {
+    GK(cudaMemsetAsync(target.p, 0, n, G.st));
+    GK(cudaMemsetAsync(target.p + witness, 1, 1, G.st));
+    std::vector<uint32_t> leg;
+    GR(bfs_path(G, nullptr, at, inscc.p, target.p, par.p, walk.p, leg));
+    cycle.insert(cycle.end(), leg.begin() + 1, leg.end() - 1);
+  } else if (cycle.size() > 1) {
+    cycle.pop_back();
+  }
+  GR(G.elapsed(&out->lasso_ms));
+  out->prefix_len = (uint32_t)prefix.size();
+  out->cycle_len = (uint32_t)cycle.size();
+  if ((uint64_t)prefix.size() + cycle.size() > lasso_cap) return TLAG_EOVERFLOW;
+  if (lasso_out) {
+    memcpy(lasso_out, prefix.data(), prefix.size() * 4);
+    memcpy(lasso_out + prefix.size(), cycle.data(), cycle.size() * 4);
+  }
   return TLAG_OK;
 }

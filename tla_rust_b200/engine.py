@@ -68,6 +68,17 @@ class GraphInfo(C.Structure):
         return {f: getattr(self, f) for f, _ in self._fields_}
 
 
+class LabelProgram(C.Structure):
+    _fields_ = [("code", C.c_void_p), ("code_len", C.c_uint32), ("entry_states", C.c_uint32), ("entry_edges", C.c_uint32),
+                ("n_state_preds", C.c_uint32), ("n_edge_preds", C.c_uint32), ("cpool", C.c_void_p), ("cpool_len", C.c_uint32),
+                ("en_bit", C.c_uint8 * 32), ("nen_bit", C.c_uint8 * 32)]
+
+
+class GraphDev(C.Structure):
+    _fields_ = [("n_states", C.c_uint64), ("n_edges", C.c_uint64), ("off", C.c_uint64), ("dst", C.c_uint64),
+                ("state_label", C.c_uint64), ("edge_label", C.c_uint64), ("n_init", C.c_uint64), ("device", C.c_int32)]
+
+
 class SimParams(C.Structure):
     _fields_ = [("seed", C.c_uint64), ("first_walk", C.c_uint64), ("num_walks", C.c_uint64), ("depth", C.c_uint32),
                 ("flags", C.c_uint32)]
@@ -88,7 +99,7 @@ EXPORTS = ["tlag_create", "tlag_seed", "tlag_step", "tlag_run", "tlag_result_now
            "tlag_frontier", "tlag_expand_route", "tlag_insert_records", "tlag_advance_level",
            "tlag_p2p_init", "tlag_p2p_attach", "tlag_p2p_level", "tlag_p2p_rollback", "tlag_read_link", "tlag_set_rank", "tlag_set_owner_words",
            "tlag_simulate", "tlag_sim_trace", "tlag_sim_read", "tlag_sim_digest",
-           "tlag_build_graph", "tlag_read_graph", "tlag_graph_digest"]
+           "tlag_build_graph", "tlag_read_graph", "tlag_graph_digest", "tlag_label_graph", "tlag_graph_view"]
 
 
 def build_library(verbose=False):
@@ -417,6 +428,28 @@ class Engine:
                                         dst.ctypes.data_as(C.c_void_p), act.ctypes.data_as(C.c_void_p)), "tlag_read_graph")
         return off, dst, act
 
+    def label_graph(self, img, en=None, nen=None) -> float:
+        """Label the state graph with a label image (compile/lower.py compile_labels).  en / nen: {edge bit: state bit} of
+        the ENABLED bits and their complements derived from the edge labels.  -> device ms"""
+        code = np.ascontiguousarray(img.code, dtype=np.uint64)
+        cpool = np.ascontiguousarray(img.cpool if len(img.cpool) else [0], dtype=np.int32)
+        eb, nb = (C.c_uint8 * 32)(*([0xFF] * 32)), (C.c_uint8 * 32)(*([0xFF] * 32))
+        for b, sb in (en or {}).items():
+            eb[b] = sb
+        for b, sb in (nen or {}).items():
+            nb[b] = sb
+        lp = LabelProgram(code.ctypes.data, len(code), img.entries["states"], img.entries["edges"], img.n_states,
+                          img.n_edges, cpool.ctypes.data, len(img.cpool), eb, nb)
+        ms = C.c_float()
+        self._ck(self.L.tlag_label_graph(self.h, C.byref(lp), C.byref(ms)), "tlag_label_graph")
+        return float(ms.value)
+
+    def graph_view(self) -> GraphDev:
+        """The state graph and its labels as device pointers (include/tlag.h: tlag_graph_view)"""
+        v = GraphDev()
+        self._ck(self.L.tlag_graph_view(self.h, C.byref(v)), "tlag_graph_view")
+        return v
+
     def graph_digest(self):
         x, s_ = C.c_uint64(), C.c_uint64()
         self._ck(self.L.tlag_graph_digest(self.h, C.byref(x), C.byref(s_)), "tlag_graph_digest")
@@ -570,6 +603,46 @@ def fair_cycles(n_states, src, dst, edge_label=None, state_label=None, state_mas
                 "tlag_fair_cycles")
     return {"violated": bool(r.violated), "witness": None if r.witness == NO_SCC else int(r.witness),
             "fair_sccs": int(r.fair_sccs), "rounds": int(r.rounds), "device_ms": float(r.device_ms), "scc": out}
+
+
+class TlagLiveQuery(C.Structure):
+    _fields_ = [("fair", C.c_void_p), ("n_fair", C.c_uint32), ("flags", C.c_uint32), ("keep_set", C.c_uint32),
+                ("keep_clear", C.c_uint32), ("edge_drop", C.c_uint32), ("need_clear", C.c_uint32), ("seed_set", C.c_uint32),
+                ("seed_clear", C.c_uint32), ("seed_rows", C.c_uint64)]
+
+
+class TlagLiveResult(C.Structure):
+    _fields_ = [("violated", C.c_int32), ("witness", C.c_uint32), ("fair_sccs", C.c_uint64), ("rounds", C.c_uint32),
+                ("prefix_len", C.c_uint32), ("cycle_len", C.c_uint32), ("reserved", C.c_uint32), ("check_ms", C.c_float),
+                ("lasso_ms", C.c_float)]
+
+
+LIVE_SEEDS, LIVE_ANY_SEED = 1, 2
+
+
+def live_check(view, fairness=(), keep_set=0, keep_clear=0, edge_drop=0, need_clear=0, seed_set=0, seed_clear=0,
+               seed_rows=0, flags=0, lasso_cap=1 << 16):
+    """Obligation check on an engine's labelled graph (include/tlag.h: tlag_live_check).  view: Engine.graph_view();
+    fairness: (kind "WF"/"SF", ENABLED state bit, action edge bit) triples.
+    -> dict(violated, witness, fair_sccs, rounds, check_ms, lasso_ms, prefix [rows], cycle [rows])"""
+    L = _graph_lib()
+    fair = (TlagFairness * max(1, len(fairness)))(*[TlagFairness(FAIR_KINDS[k], en, act, 0) for k, en, act in fairness])
+    q = TlagLiveQuery(C.addressof(fair), len(fairness), flags, keep_set, keep_clear, edge_drop, need_clear, seed_set,
+                      seed_clear, seed_rows)
+    while True:
+        lasso = np.zeros(lasso_cap, dtype=np.uint32)
+        r = TlagLiveResult()
+        rc = L.tlag_live_check(C.byref(view), C.byref(q), lasso.ctypes.data_as(C.c_void_p), C.c_uint32(lasso_cap),
+                               C.byref(r))
+        if rc == -5 and r.prefix_len + r.cycle_len > lasso_cap:     # TLAG_EOVERFLOW: the lasso's length is set
+            lasso_cap = int(r.prefix_len + r.cycle_len)
+            continue
+        _graph_call(L, rc, "tlag_live_check")
+        break
+    p, c = int(r.prefix_len), int(r.cycle_len)
+    return {"violated": bool(r.violated), "witness": None if r.witness == NO_SCC else int(r.witness),
+            "fair_sccs": int(r.fair_sccs), "rounds": int(r.rounds), "check_ms": float(r.check_ms),
+            "lasso_ms": float(r.lasso_ms), "prefix": lasso[:p].tolist(), "cycle": lasso[p:p + c].tolist()}
 
 
 class ProbeOnlyModel:

@@ -5,6 +5,7 @@ from __future__ import annotations
 from .values import fmt
 
 OK, INVARIANT, ASSERT, DEADLOCK, EVAL_ERROR, PROPERTY = "ok", "invariant", "assert", "deadlock", "eval_error", "property"
+LIVENESS = "liveness"
 
 
 class CheckResult:
@@ -22,6 +23,7 @@ class CheckResult:
         self.levels = []         # distinct states discovered per level (for parity debugging)
         self.seconds = 0.0
         self.extra = {}
+        self.back_to = None      # LIVENESS: (1-based state the cycle goes back to, action label) or None: stuttering
 
     def summary(self):
         return dict(verdict=self.verdict, generated=self.generated, distinct=self.distinct,
@@ -67,11 +69,26 @@ def format_result(res: CheckResult, var_order, module):
             out.append(f"Error: Invariant {res.invariant} is violated.")
         elif res.verdict == DEADLOCK:
             out.append("Error: Deadlock reached.")
+        elif res.verdict == LIVENESS:
+            out.append("Error: Temporal properties were violated.")
+            out.append("")
+            out.append("Error: The following behavior constitutes a counter-example:")
+            out.append("")
+            for i, (st, act) in enumerate(res.trace, 1):
+                out.append(f"State {i}: {action_label(act, module)}")
+                out.append(format_state(st, var_order))
+                out.append("")
+            if res.back_to is None:
+                out.append(f"State {len(res.trace) + 1}: Stuttering")
+            else:
+                out.append(f"Back to state {res.back_to[0]}: {action_label(res.back_to[1], module)}")
+            out.append("")
         elif res.verdict == PROPERTY:
             out.append(f"Error: Action property {res.invariant} is violated.")
         else:
             out.append(f"Error: {res.error_text}")
-        out.append(format_trace(res, var_order, module))
+        if res.verdict != LIVENESS:
+            out.append(format_trace(res, var_order, module))
         if res.error_positions:
             out.append("Error: The error occurred when TLC was evaluating the nested")
             out.append("expressions at the following positions:")

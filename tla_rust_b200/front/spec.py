@@ -264,6 +264,61 @@ def _has_temporal(n, ctx, seen=None, depth=0):
     return any(_has_temporal(x, ctx, seen, depth) for x in n.a)
 
 
+def _state_pred(n, ctx, seen=None, depth=0):
+    """n is a state predicate: no temporal operator, prime, ENABLED, UNCHANGED or action form, definitions included"""
+    if not isinstance(n, Node):
+        if isinstance(n, (tuple, list)):
+            return all(_state_pred(x, ctx, seen, depth) for x in n)
+        return True
+    if n.k in _TEMPORAL or n.k in ("prime", "enabled", "unchanged", "aangle", "abox"):
+        return False
+    if n.k == "bin" and n.a[0] in ("~>", "-+->", "\\cdot"):
+        return False
+    if n.k in ("id", "app") and depth < 8 and isinstance(n.a[0], str):
+        d = ctx.defs.get(n.a[0])
+        if n.k == "app" and not _state_pred(n.a[1], ctx, seen, depth):
+            return False
+        if d is not None:
+            seen = seen or set()
+            if n.a[0] in seen:
+                return True
+            seen.add(n.a[0])
+            return _state_pred(d[0].body, d[1], seen, depth + 1)
+        return True
+    if n.k == "let":
+        return _state_pred(n.a[1], ctx, seen, depth)
+    return all(_state_pred(x, ctx, seen, depth) for x in n.a)
+
+
+class Pred:
+    """A state predicate, or an action (<<A>>_v), with the context and the bound variables it is evaluated in"""
+
+    def __init__(self, node, ctx, env):
+        self.node, self.ctx, self.env = node, ctx, dict(env)
+
+    def key(self):
+        return (repr(self.node), id(self.ctx), repr(sorted(self.env.items(), key=lambda kv: kv[0])))
+
+
+class Fairness:
+    """WF_v(A) or SF_v(A): kind "WF" / "SF"; act() is <<A>>_v as a Pred"""
+
+    def __init__(self, kind, a, sub, ctx, env, loc):
+        self.kind, self.a, self.sub, self.ctx, self.env, self.loc = kind, a, sub, ctx, dict(env), loc
+
+    def act(self):
+        return Pred(Node("aangle", (self.a, self.sub), *self.loc), self.ctx, self.env)
+
+
+class Obligation:
+    """One temporal PROPERTY conjunct in normal form (DESIGN.md §7h).  kind:
+      "always" []p, "eventually" <>p, "leadsto" p ~> q, "inf" a disjunction of terms ("ie", X) []<>X, ("iea", A)
+      []<><<A>>_v, ("eg", X) <>[]X, "wf" / "sf" a fairness condition asserted as a property (fair)."""
+
+    def __init__(self, name, loc, kind, p=None, q=None, terms=(), fair=None):
+        self.name, self.loc, self.kind, self.p, self.q, self.terms, self.fair = name, loc, kind, p, q, list(terms), fair
+
+
 class Model:
     """A checkable model: root context + Init / Next / invariants, after cfg application."""
 
@@ -326,7 +381,8 @@ class Model:
         self.next_node = None
         self.next_ctx = ctx
         self.vars = list(ctx.vars)
-        self.fairness_ignored = False
+        self.fairness = []
+        self.fairness_unknown = []      # source locations of SPECIFICATION temporal conjuncts outside the supported forms
         if cfg.specification:
             self._split_spec(Node("id", (cfg.specification,)), ctx)
         else:
@@ -348,49 +404,81 @@ class Model:
         for nm in cfg.action_constraints:
             d, c = self._def(nm)
             self.action_constraints.append((nm, d.body, c))
-        # PROPERTYs: the safety part  Init2 /\ [][Next2]_v2  becomes a refinement obligation: Init => Init2 and
-        # every transition satisfies [Next2]_v2 (MCPaxos.cfg:12, MCVoting.cfg:9, HourClock2.cfg:9); the
-        # liveness part (fairness, <>, ~>) is out of scope and ignored with a warning.
+        # PROPERTYs: the safety part  Init2 /\\ [][Next2]_v2  becomes a refinement obligation: Init => Init2 and
+        # every transition satisfies [Next2]_v2 (MCPaxos.cfg:12, MCVoting.cfg:9, HourClock2.cfg:9); each temporal
+        # conjunct in one of the forms of DESIGN.md §7h becomes a liveness obligation (checked on the state graph), any
+        # other one is ignored with a warning that names it.
         self.properties = list(cfg.properties)
         self.refinements = []
+        self.obligations = []
         for nm in cfg.properties:
             d, c = self._def(nm)
-            acc = {"init": [], "next": None, "sub": None, "ctx": None, "live": False}
+            acc = {"init": [], "next": None, "sub": None, "ctx": None, "name": nm}
             self._split_prop(d.body, c, acc)
-            if acc["live"]:
-                self.warnings.append(f"PROPERTY {nm}: temporal (liveness) conjuncts are not checked")
             if acc["next"] is not None or acc["init"]:
                 self.refinements.append((nm, acc["init"], acc["next"], acc["sub"], acc["ctx"]))
         self.symmetry = cfg.symmetry
         self.check_deadlock = True if cfg.check_deadlock is None else cfg.check_deadlock
 
-    def _split_spec(self, n, ctx):
-        """Decompose  Init /\\ [][Next]_vars /\\ fairness  (SURVEY.md §3.2)."""
+    def _conjuncts(self, n, ctx, env=None):
+        """The conjuncts of n, as (node, ctx, env): through conjunction lists, parameterless definitions and instance
+        selectors whose bodies are temporal, and  \\A x \\in S : body  with a temporal body and S a finite constant
+        set (one conjunct per element, x bound in env)."""
+        env = env or {}
         if n.k == "and":
             for x in n.a[0]:
-                self._split_spec(x, ctx)
+                yield from self._conjuncts(x, ctx, env)
             return
-        if n.k == "box" and n.a[0].k == "abox":
-            if self.next_node is not None:
-                raise SpecError("specification has more than one [][Next]_v conjunct")
-            self.next_node = n.a[0].a[0]
-            self.next_ctx = ctx
-            self.subscript = n.a[0].a[1]
-            return
-        if n.k == "id":
+        if n.k == "id" and n.a[0] not in env:
             d = ctx.defs.get(n.a[0])
             if d is not None and not d[0].params and _has_temporal(d[0].body, d[1]):
-                self._split_spec(d[0].body, d[1])
+                yield from self._conjuncts(d[0].body, d[1])
                 return
         if n.k == "sel":
             r = self.ev.resolve_sel(n.a[0], {}, Fr(ctx))
-            if r[0] == "def" and _has_temporal(r[1].body, r[2]):
-                self._split_spec(r[1].body, r[2])
+            if r[0] == "def" and not r[1].params and _has_temporal(r[1].body, r[2]):
+                yield from self._conjuncts(r[1].body, r[2])
                 return
-        if _has_temporal(n, ctx):
-            self.fairness_ignored = True
-            return
-        self.init_nodes.append((n, ctx))
+        if n.k == "bin" and n.a[0] == "=>" and _has_temporal(n.a[2], ctx) and not _has_temporal(n.a[1], ctx):
+            try:                 # a constant-level guard (InnerSerial.tla:116): the conjunct applies when it holds
+                g = self.ev.eval(n.a[1], env, Fr(ctx))
+            except EvalError:
+                g = None
+            if g is True:
+                yield from self._conjuncts(n.a[2], ctx, env)
+                return
+            if g is False:
+                return
+        if n.k == "forall" and _has_temporal(n.a[1], ctx):
+            try:
+                envs = list(self.ev.iter_bounds(n.a[0], env, Fr(ctx)))
+            except EvalError:
+                envs = None
+            if envs is not None:
+                for env2 in envs:
+                    yield from self._conjuncts(n.a[1], ctx, env2)
+                return
+        yield n, ctx, env
+
+    def _split_spec(self, n, ctx):
+        """Decompose  Init /\\ [][Next]_vars /\\ fairness  (SURVEY.md §3.2)."""
+        for x, c, env in self._conjuncts(n, ctx):
+            if x.k == "box" and x.a[0].k == "abox":
+                if self.next_node is not None:
+                    raise SpecError("specification has more than one [][Next]_v conjunct")
+                self.next_node = x.a[0].a[0]
+                self.next_ctx = c
+                self.subscript = x.a[0].a[1]
+            elif x.k in ("wf", "sf"):
+                self.fairness.append(Fairness(x.k.upper(), x.a[1], x.a[0], c, env, x.loc()))
+            elif _has_temporal(x, c):
+                # the fairness the spec states is not known: a liveness verdict could be wrong either way
+                if x.loc() not in self.fairness_unknown:
+                    self.fairness_unknown.append(x.loc())
+                    self.warnings.append(f"SPECIFICATION {self.cfg.specification}: the temporal conjunct at line "
+                                         f"{x.line}, col {x.col} is not a WF or SF condition in a supported form")
+            else:
+                self.init_nodes.append((x, c))
 
     def symmetry_group(self):
         """Non-identity elements of the group generated by the SYMMETRY set (Paxos/MCPaxos.cfg:13:
@@ -413,27 +501,74 @@ class Model:
         return permutation_group(perms)
 
     def _split_prop(self, n, ctx, acc):
-        if n.k == "and":
-            for x in n.a[0]:
-                self._split_prop(x, ctx, acc)
-            return
-        if n.k == "box" and n.a[0].k == "abox":
-            acc["next"], acc["sub"], acc["ctx"] = n.a[0].a[0], n.a[0].a[1], ctx
-            return
-        if n.k == "id":
-            d = ctx.defs.get(n.a[0])
-            if d is not None and not d[0].params and _has_temporal(d[0].body, d[1]):
-                self._split_prop(d[0].body, d[1], acc)
-                return
-        if n.k == "sel":
-            r = self.ev.resolve_sel(n.a[0], {}, Fr(ctx))
-            if r[0] == "def" and _has_temporal(r[1].body, r[2]):
-                self._split_prop(r[1].body, r[2], acc)
-                return
-        if _has_temporal(n, ctx):
-            acc["live"] = True
-            return
-        acc["init"].append((n, ctx))
+        for x, c, env in self._conjuncts(n, ctx):
+            if x.k == "box" and x.a[0].k == "abox":
+                acc["next"], acc["sub"], acc["ctx"] = x.a[0].a[0], x.a[0].a[1], c
+            elif _has_temporal(x, c):
+                ob = self._obligation(x, c, env, acc["name"])
+                if ob is None and x.loc() not in acc.setdefault("warned", set()):
+                    acc["warned"].add(x.loc())
+                    self.warnings.append(f"PROPERTY {acc['name']}: the temporal (liveness) conjunct at line {x.line}, "
+                                         f"col {x.col} is not checked (not one of the forms of DESIGN.md §7h)")
+                elif ob is not None:
+                    self.obligations.append(ob)
+            else:
+                acc["init"].append((x, c))
+
+    def _unfold(self, n, ctx):
+        """n with parameterless definitions and instance selectors replaced by their bodies (one level at a time)"""
+        for _ in range(16):
+            if n.k == "id" and ctx.defs.get(n.a[0]) is not None and not ctx.defs[n.a[0]][0].params:
+                n, ctx = ctx.defs[n.a[0]][0].body, ctx.defs[n.a[0]][1]
+            elif n.k == "sel":
+                r = self.ev.resolve_sel(n.a[0], {}, Fr(ctx))
+                if r[0] != "def" or r[1].params:
+                    break
+                n, ctx = r[1].body, r[2]
+            else:
+                break
+        return n, ctx
+
+    def _obligation(self, n, ctx, env, name):
+        """The liveness obligation of a temporal PROPERTY conjunct (DESIGN.md §7h), or None outside its forms"""
+        sp = lambda x, c: _state_pred(x, c) and Pred(x, c, env)
+
+        def term(x, c):          # []<>X, []<><<A>>_v, <>[]X -> ("ie" | "iea" | "eg", Pred)
+            x, c = self._unfold(x, c)
+            if x.k == "box":
+                y, c2 = self._unfold(x.a[0], c)
+                if y.k == "diamond":
+                    z = y.a[0]
+                    if z.k == "aangle" and not _has_temporal(z, c2):
+                        return "iea", Pred(z, c2, env)
+                    p = sp(z, c2)
+                    return p and ("ie", p)
+            if x.k == "diamond":
+                y, c2 = self._unfold(x.a[0], c)
+                if y.k == "box":
+                    p = sp(y.a[0], c2)
+                    return p and ("eg", p)
+            return None
+
+        loc = n.loc()
+        if n.k in ("wf", "sf"):
+            return Obligation(name, loc, n.k, fair=Fairness(n.k.upper(), n.a[1], n.a[0], ctx, env, loc))
+        if n.k == "bin" and n.a[0] == "~>":
+            p, q = sp(n.a[1], ctx), sp(n.a[2], ctx)
+            return Obligation(name, loc, "leadsto", p=p, q=q) if p and q else None
+        t = term(n, ctx)
+        if t:
+            return Obligation(name, loc, "inf", terms=[t])
+        if n.k == "or":
+            terms = [term(x, ctx) for x in n.a[0]]
+            return Obligation(name, loc, "inf", terms=terms) if all(terms) else None
+        if n.k == "box":
+            p = sp(n.a[0], ctx)
+            return Obligation(name, loc, "always", p=p) if p else None
+        if n.k == "diamond":
+            p = sp(n.a[0], ctx)
+            return Obligation(name, loc, "eventually", p=p) if p else None
+        return None
 
     def in_model(self, st) -> bool:
         """CONSTRAINTs on a state (host side: used for the initial states; on successors the device evaluates them)"""
